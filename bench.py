@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- xRT (audio seconds / wall seconds) + encode ms of the Whisper hot path on B200.
+"""bench.py -- xRT (audio seconds / wall seconds) + encode ms of the Whisper hot path on H100.
 
 Workload (BASELINE.json configs[3]): large-v3 Q5_0, synthetic weights (no checkpoints offline), a batch of 64 independent
 30 s chunks per GPU, greedy decode (best_of=1, no temperature fallback), text tokens only (see full_params).  A "step" is one pass over the
@@ -16,6 +16,10 @@ rank's 64 chunks (all 64 sequences advance in lock-step: one batched encoder pas
 
 `--impl reference` times the reference's own CPU implementation (oracle/_ref, unmodified whisper.cpp) on a bounded
 sample of the same workload (1 chunk per step) with all host threads.
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step: per chunk, the decoded token ids and their
+probabilities (DIR/tokens.npy float64, DIR/token_p.npy float32, both [chunks][max tokens] padded with -1) and the token counts
+(DIR/n_tokens.npy float64).  Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -39,17 +43,21 @@ MODEL_CFG = "large-v3"
 WORKLOAD = "large-v3 Q5_0 (synthetic weights), %d x 30 s chunks per GPU, greedy best_of=1, no fallback, no_timestamps (224 tokens per chunk)" % CHUNKS_PER_GPU
 
 
+# NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense FP16 / BF16 tensor rate; upper bounds, not measured rates
+H100_HBM_GBS, H100_F16_TFLOPS = 3350.0, 989.0
+
+
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             j = json.load(f)
-        return float(j.get("hbm_gbs", 6650.0)), float(j.get("bf16_tflops_sustained", 1400.0)), "measured"
-    return 6650.0, 1400.0, "fallback"
+        return float(j.get("hbm_gbs", H100_HBM_GBS)), float(j.get("bf16_tflops_sustained", H100_F16_TFLOPS)), "measured"
+    return H100_HBM_GBS, H100_F16_TFLOPS, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons during the timed region"""
 
     def __init__(self, index):
         self.index = index
@@ -72,6 +80,7 @@ class ClockSampler:
     def stop(self):
         if self.proc:
             self.proc.terminate()
+            self.proc.wait()
         sm = [float(r[0]) for r in self.rows if r and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         reasons = set()
@@ -231,7 +240,7 @@ def _timings(L, ctx):
 
 
 def run_config2(args, local):
-    """BASELINE configs[1]: base.en Q5_0, single B200, ONE 30 s chunk, encoder + greedy decode with timestamps, through whisper_full"""
+    """BASELINE configs[1]: base.en Q5_0, single GPU, ONE 30 s chunk, encoder + greedy decode with timestamps, through whisper_full"""
     import torch
     pkg = load_pkg(); synth = pkg.synth
     model = synth.cached_model("base.en", synth.Q5_0, seed=4, tag="s4")
@@ -249,7 +258,7 @@ def run_config2(args, local):
             toks = sum(L.whisper_full_n_tokens(eng.ctx, i) for i in range(L.whisper_full_n_segments(eng.ctx)))
     dt = float(np.mean(times))
     out = {"metric": "xRT (audio-s/wall-s)", "value": CHUNK_SECONDS / dt, "unit": "x real time", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * dt,
-           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 tcgen05 (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
+           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 wgmma (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
            "config": {"workload": "BASELINE configs[1]: base.en Q5_0 (synthetic weights), one 30 s chunk, greedy best_of=1, timestamps on, whisper_full with host PCM"},
            "encode_ms": tm["encode_ms"], "decode_ms_per_token": tm["decode_ms"], "prompt_ms_per_token": tm["prompt_ms"], "decoded_tokens": toks,
            "e2e": {"value": CHUNK_SECONDS / dt, "unit": "x real time", "h2d_bytes_per_step": pcm.numel() * 4, "d2h_bytes_per_step": None}}
@@ -258,7 +267,7 @@ def run_config2(args, local):
 
 
 def run_config3(args, local):
-    """BASELINE configs[2]: large-v3 Q4_K, single B200, beam_size 5, ONE 30-minute synthetic clip (60 x the 30 s generator, seeds 1234+i), whisper_full"""
+    """BASELINE configs[2]: large-v3 Q4_K, single GPU, beam_size 5, ONE 30-minute synthetic clip (60 x the 30 s generator, seeds 1234+i), whisper_full"""
     import torch
     pkg = load_pkg(); synth = pkg.synth
     model = synth.cached_model("large-v3", synth.Q4_K, seed=0, fast_pool=True)
@@ -276,7 +285,7 @@ def run_config3(args, local):
     tm = _timings(L, eng.ctx)
     audio = pcm.numel() / 16000.0
     out = {"metric": "xRT (audio-s/wall-s)", "value": audio / dt, "unit": "x real time", "n_gpus": 1, "steps": 1, "warmup": 0, "ms_per_step": 1e3 * dt,
-           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 tcgen05 (encode) / int8 block dot (decode), f32 accumulate", "data": "synthetic",
+           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 wgmma (encode) / int8 block dot (decode), f32 accumulate", "data": "synthetic",
            "config": {"workload": "BASELINE configs[2]: large-v3 Q4_K (synthetic weights), beam_size 5, one %.0f-minute clip, whisper_full with host PCM (sequential windows: one stream)" % (audio / 60)},
            "encode_ms": tm["encode_ms"], "batchd_ms_per_token": tm["batchd_ms"], "sample_ms": tm["sample_ms"], "windows": c1[5] - c0[5], "decode_passes": c1[0] - c0[0], "rows_per_pass": (c1[1] - c0[1]) / max(1.0, c1[0] - c0[0]),
            "decoded_tokens": sum(L.whisper_full_n_tokens(eng.ctx, i) for i in range(L.whisper_full_n_segments(eng.ctx))),
@@ -327,7 +336,7 @@ def run_config5(args, rank, local, world):
     if rank == 0:
         best = max(rows, key=lambda r: r["xrt"])
         out = {"metric": "xRT (audio-s/wall-s)", "value": best["xrt"], "unit": "x real time", "n_gpus": world, "steps": args.steps, "warmup": 1, "ms_per_step": best["ms_per_wave"],
-               "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 tcgen05 (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
+               "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 wgmma (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
                "config": {"workload": "BASELINE configs[4]: large-v3-turbo Q8_0 (synthetic weights), sweep of concurrent 30 s chunks (threads x whisper_full_with_state, whisper.h only), greedy, no_timestamps"},
                "sweep": rows, "latency_note": "chunk latency of rank 0's chunks (submit -> transcript), rank-local clocks",
                "e2e": {"value": best["xrt"], "unit": "x real time", "h2d_bytes_per_step": None, "d2h_bytes_per_step": None}}
@@ -343,6 +352,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy (default workload)")
     ap.add_argument("--chunks", type=int, default=CHUNKS_PER_GPU, help="chunks per GPU (weak scaling)")
     ap.add_argument("--chunks-total", type=int, default=0, help="strong scaling: this many chunks in total, split over the ranks")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -399,7 +409,26 @@ def main():
     concat = torch.from_numpy(np.concatenate(pcms)).pin_memory()       # whisper_full_parallel input: one host buffer, sliced by the library
     states = []
 
-    def run_pass(mode):
+    def dump_outputs(outs):
+        """token ids / probabilities of every chunk of one step (what whisper_full_get_token_data_from_state hands a caller)"""
+        L.whisper_full_get_token_data_from_state.restype = pkg.TokenData
+        L.whisper_full_get_token_data_from_state.argtypes = [vp, C.c_int, C.c_int]
+        toks = [[] for _ in range(n_chunks)]; probs = [[] for _ in range(n_chunks)]
+        for c in range(n_chunks):
+            for i in range(L.whisper_full_n_segments_from_state(outs[c])):
+                for j in range(L.whisper_full_n_tokens_from_state(outs[c], i)):
+                    td = L.whisper_full_get_token_data_from_state(outs[c], i, j)
+                    toks[c].append(td.id); probs[c].append(td.p)
+        width = max(1, max(len(t) for t in toks))
+        tok = np.full((n_chunks, width), -1.0, np.float64); prb = np.full((n_chunks, width), -1.0, np.float32)
+        for c in range(n_chunks):
+            tok[c, :len(toks[c])] = toks[c]; prb[c, :len(probs[c])] = probs[c]
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "tokens.npy"), tok)
+        np.save(os.path.join(args.dump_outputs, "token_p.npy"), prb)
+        np.save(os.path.join(args.dump_outputs, "n_tokens.npy"), np.array([len(t) for t in toks], np.float64))
+
+    def run_pass(mode, keep=False):
         """one step = all chunks of this rank.  mode "device": PCM resident in HBM (library queue driver); "parallel": one
         whisper_full_parallel call on host PCM; "threads": one caller thread per chunk, whisper_full_with_state on its own state"""
         if mode == "parallel":
@@ -425,10 +454,12 @@ def main():
         rc = L.wb200_full_batch_ex(eng.ctx, p, dev_ptrs, n_arr, n_chunks, outs, 1)
         assert rc == 0, (rc, L.wb200_last_error())
         last["tokens"] = sum(count_tokens(L, outs[i]) for i in range(n_chunks))
+        if keep:                                                        # the caller reads and frees them
+            return outs
         for i in range(n_chunks):
             L.whisper_free_state(outs[i])
 
-    def timed(mode, steps, warmup):
+    def timed(mode, steps, warmup, capture=False):
         for _ in range(warmup):
             run_pass(mode)
         if world > 1:
@@ -437,10 +468,16 @@ def main():
         h0, d0 = C.c_uint64(), C.c_uint64(); L.wb200_traffic(C.byref(h0), C.byref(d0))
         n0 = eng.launch_count()
         t0 = time.perf_counter()
-        for _ in range(steps):
-            run_pass(mode)
+        outs = None
+        for i in range(steps):
+            outs = run_pass(mode, keep=capture and i == steps - 1)
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
+        if outs is not None:                                            # the last step's states: outputs written, then released
+            if rank == 0:
+                dump_outputs(outs)
+            for i in range(n_chunks):
+                L.whisper_free_state(outs[i])
         h1, d1 = C.c_uint64(), C.c_uint64(); L.wb200_traffic(C.byref(h1), C.byref(d1))
         launches = eng.launch_count() - n0
         dt = max_over_ranks(dt, world)
@@ -455,7 +492,7 @@ def main():
     for _ in range(args.warmup):
         run_pass("device")
     c0 = counters()
-    dt_res, launches, _, _ = timed("device", args.steps, 0)
+    dt_res, launches, _, _ = timed("device", args.steps, 0, capture=bool(args.dump_outputs))
     c1 = counters()
     clocks = sampler.stop()
     cd = [b - a for a, b in zip(c0, c1)]
@@ -472,6 +509,11 @@ def main():
     tokens_e2e = last["tokens"]
     dt_thr, _, h2d_t, d2h_t = timed("threads", args.steps, max(1, args.warmup))
     e2e_threads = audio_s / dt_thr
+    # released before the passes below: next to their states, another 64 would grow the context's pool to 150 windows of cross K/V
+    # (37.7 GB for large-v3), more than an 80 GB card holds beside the rest
+    for st in states:
+        L.whisper_free_state(st)
+    states.clear()
 
     # ---- encode ms of ONE 30 s window (whisper-bench "Enc." semantics: conv + encoder + cross, bench.cpp:63-150) on the default state
     st0 = L.wb200_ctx_state(eng.ctx)
@@ -518,8 +560,8 @@ def main():
 
     out = {"metric": "xRT (audio-s/wall-s)", "value": value, "unit": "x real time", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
            "ms_per_step": 1e3 * dt_res / args.steps, "higher_is_better": True, "scaling": scaling, "vs_baseline": None,
-           "dtype": "f16 tcgen05 (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
-           "config": {"workload": WORKLOAD, "chunks_per_gpu": n_chunks, "decode": "lock-step batch of up to 64 sequences per GPU, one persistent cooperative kernel per token step", "l2": "weights (1.08 GB) + KV (0.3 GB/sequence) streamed every step exceed the 126 MB L2",
+           "dtype": "f16 wgmma (encode) / int8 mma block dot (decode), f32 accumulate", "data": "synthetic",
+           "config": {"workload": WORKLOAD, "chunks_per_gpu": n_chunks, "decode": "lock-step batch of up to 64 sequences per GPU, one persistent cooperative kernel per token step", "l2": "weights (1.08 GB) + KV (0.3 GB/sequence) streamed every step exceed the 50 MB L2",
                       "timing": "host wall clock between device synchronisations around whole steps (a step contains host control flow), max over ranks; per-kernel numbers from CUDA events on the launching stream"},
            "encode_ms": float(enc[1] + enc[2] + enc[3]), "encode_ms_parts": {"mel": float(enc[0]), "conv": float(enc[1]), "encoder": float(enc[2]), "cross": float(enc[3])},
            "decoded_tokens_per_step": tokens, "engine": engine_stats, "clocks": clocks, "gpu_launches": int(launches),
@@ -538,7 +580,7 @@ def main():
         L.wb200_profile_collect(ms, ln, by, fl)
         L.wb200_profile_enable(0)
         hbm, tf, how = measured_peaks()
-        names = ["tcgen05_gemm", "decode_pass_persistent", "decode_attention", "other"]
+        names = ["wgmma_gemm", "decode_pass_persistent", "decode_attention", "other"]
         classes = {names[i]: {"ms": ms[i], "launches": int(ln[i]), "GBps": (by[i] / 1e9) / (ms[i] / 1e3) if ms[i] > 0 else 0.0,
                               "TFLOPs": (fl[i] / 1e12) / (ms[i] / 1e3) if ms[i] > 0 else 0.0} for i in range(4)}
         dom = max(range(3), key=lambda i: ms[i])
@@ -546,16 +588,6 @@ def main():
             roof = {"kernel": names[0], "bound": "tensor", "achieved": classes[names[0]]["TFLOPs"], "peak": tf, "unit": "TFLOP/s", "frac": classes[names[0]]["TFLOPs"] / tf, "traffic": None, "peak_source": how + " (sustained bf16)"}
         else:
             roof = {"kernel": names[dom], "bound": "hbm", "achieved": classes[names[dom]]["GBps"], "peak": hbm, "unit": "GB/s", "frac": classes[names[dom]]["GBps"] / hbm, "traffic": None, "peak_source": how}
-        # DRAM traffic of one launch of the dominant kernel from the committed `ncu --set full` capture (profiles/), if it is the same kernel
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_ncu_decode_pass.json")) as f:
-                cap = json.load(f)
-            if dom == 1 and cap.get("rows") == min(n_chunks, 64):
-                roof["traffic"] = cap["dram_bytes_read"] + cap["dram_bytes_write"]
-                roof["traffic_source"] = "profiles/r02_ncu_decode_pass.json (one launch, %d rows)" % cap["rows"]
-                roof["algorithmic_bytes_per_launch"] = (by[dom] / ln[dom]) if ln[dom] else None
-        except Exception:  # noqa: BLE001
-            pass
         out["roofline"] = roof
         out["kernel_classes"] = classes
         if not args.no_cpu_baseline:

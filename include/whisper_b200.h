@@ -1,5 +1,5 @@
 /*
- * whisper_b200.h -- C ABI of libwhisper_b200.so, the B200-native (sm_100a) Whisper engine.
+ * whisper_b200.h -- C ABI of libwhisper_b200.so, the CUDA-native Whisper engine for the H100 (sm_90a).
  *
  * Binary-compatible with the reference interface `include/whisper.h` of ggml-org/whisper.cpp
  * @ 233fe1fc: same exported names, same by-value struct layouts, same return-code conventions,
@@ -436,7 +436,7 @@ WB_EXPORT int wb200_state_device(struct whisper_state * state);
 /* stage PCM in HBM ahead of time: a following whisper_full_with_state(ctx, state, params, NULL, n_samples) (or
  * whisper_pcm_to_mel_with_state with samples == NULL) then starts from the device-resident samples (bench.py `value`) */
 WB_EXPORT int wb200_pcm_upload(struct whisper_state * state, const float * samples, int n_samples);
-/* per-kernel-class CUDA-event timing (classes: 0 tcgen05 GEMM, 1 decode GEMV, 2 decode attention, 3 other).
+/* per-kernel-class CUDA-event timing (classes: 0 wgmma GEMM, 1 decode GEMV, 2 decode attention, 3 other).
  * enable(1) clears the accumulators; collect() synchronises the device and fills four arrays of 4 entries:
  * summed duration [ms], launches, algorithmic bytes, algorithmic flops. */
 WB_EXPORT void wb200_profile_enable(int on);

@@ -1,12 +1,11 @@
-"""End-to-end parity on the GPU: the same whisper.h calls on libwhisper_b200.so (B200) and on the UNMODIFIED reference
+"""End-to-end parity on the GPU: the same whisper.h calls on libwhisper_b200.so (H100) and on the UNMODIFIED reference
 CPU build (oracle/_ref), on synthetic-weight models written by whisper.cpp_b200/synth.py.
 
 What is compared, and why the tolerances are what they are (SURVEY.md facts 3 and 7):
   * the reference CPU path quantises ACTIVATIONS to int8 per 32/256 values before every matmul on quantised weights,
     so its own outputs carry ~1e-2 relative noise w.r.t. exact arithmetic; this engine multiplies the exact f16
-    dequantised weights on the tensor cores (encode) and mirrors the int8 path only in the decode GEMV.  Measured on
-    B200 (tests/e2e_report.py): encoder output rms error 8.6e-3 (Q5_0) / 3.2e-4 (F16) of the output rms; logits
-    rms error 1.4e-2 / 2.0e-3 of the logits' standard deviation.
+    dequantised weights on the tensor cores (encode) and mirrors the int8 path only in the decode GEMV.
+    tests/e2e_report.py prints the encoder-output and logits rms errors of each weight format.
   * token ids: random weights give near-tied logits (top-2 margin often < 0.1 std), so greedy sequences are only
     required to agree while the reference's own margin exceeds the measured logit error; teacher-forced steps are
     checked one by one with that rule, and the free-running transcripts must share a non-trivial prefix.
@@ -100,7 +99,7 @@ def test_whisper_full_beam_search_matches_reference(lib, ref, tmp_path):
     one row per live beam.  The reference draws each beam's candidates from std::discrete_distribution(probs) with a seeded
     mt19937 (whisper_sample_token_topk): tests/test_sampler_cpu.py shows this library makes bit-identical draws from identical
     probabilities, but with random weights the distribution is nearly flat (p_max ~ 0.1 over 51k ids), so the ~1e-2 logit noise
-    between the two arithmetic paths moves almost every draw to another id (measured on B200: common prefix 1 of 27 tokens).
+    between the two arithmetic paths moves almost every draw to another id.
     Asserted here: control flow (return code, segment start), valid ids and the same first token; transcript-level agreement
     of beam search needs a real checkpoint (peaked distributions) and is listed under known gaps in DESIGN.md."""
     path = _build(tmp_path, ref, "test-2l.en", F16, seed=11)
@@ -213,8 +212,8 @@ def test_persistent_decode_kernel_matches_kernel_chain(lib, ref, tmp_path, cfg, 
 
     Both run the same arithmetic (Q8_0 activation blocks, integer block dots, f16-rounded Q); they differ in f32 summation
     order (LayerNorm statistics, split-K), and a 1e-7 difference occasionally moves an activation across an int8 / f16
-    rounding boundary (measured on B200: most steps are bit-identical, the others differ by 3e-3 .. 1.2e-2 of the logits'
-    std while both stay equally far from the reference) -- so the cross-check uses the reference tolerance, requires the
+    rounding boundary (most steps are bit-identical, the others differ by a fraction of the reference tolerance while both
+    stay equally far from the reference) -- so the cross-check uses the reference tolerance, requires the
     persistent kernel to be as close to the reference as the chain, and two runs of it must agree BIT FOR BIT."""
     path = _build(tmp_path, ref, cfg, wt, seed=5)
     pcm = synth.synth_audio(seed=21, seconds=12.0)

@@ -84,10 +84,11 @@ class Script:
         np.ctypeslib.as_array(logits, (V,))[:] = x
 
 
-def make_models(tmp_path):
-    en = str(tmp_path / "s1.en.bin"); ml = str(tmp_path / "s1.multi.bin")
+def make_models(tmp_path, multilingual=True):
+    en = str(tmp_path / "s1.en.bin"); ml = str(tmp_path / "s1.multi.bin") if multilingual else None
     synth.write_model(en, (51864, 1500, 384, 6, 1, 448, 384, 6, 1, 80), F16, seed=21, vocab_from=os.path.join(DATA_DIR, "for-tests-ggml-tiny.en.bin"))
-    synth.write_model(ml, (51865, 1500, 384, 6, 1, 448, 384, 6, 1, 80), F16, seed=22, vocab_from=os.path.join(DATA_DIR, "for-tests-ggml-tiny.bin"))
+    if multilingual:
+        synth.write_model(ml, (51865, 1500, 384, 6, 1, 448, 384, 6, 1, 80), F16, seed=22, vocab_from=os.path.join(DATA_DIR, "for-tests-ggml-tiny.bin"))
     return en, ml
 
 
@@ -275,7 +276,7 @@ def test_lockstep_batch_driver_equals_reference_chunk_by_chunk(lib, ref, tmp_pat
         X.whisper_log_set.argtypes = [LOG_CB, vp]
         X.whisper_log_set(_quiet, None)
     L.wb200_dbg_scripted_context.restype = vp; L.wb200_dbg_scripted_context.argtypes = [C.c_char_p]
-    en, _ = make_models(tmp_path)
+    en, _ = make_models(tmp_path, multilingual=False)
     cp = R.whisper_context_default_params(); cp.use_gpu = False
     rctx = R.whisper_init_from_file_with_params(en.encode(), cp)
     lctx = L.wb200_dbg_scripted_context(en.encode())

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (whisper.cpp_b200/csrc/wb_gemm.cu) against a float64 contraction of the reference-dequantised
+"""wgmma GEMM (whisper.cpp_b200/csrc/wb_gemm.cu) against a float64 contraction of the reference-dequantised
 weights (ggml-quants.c dequantize_row_*) and the f16-rounded activations the kernel consumes.
 
 Tolerance: the kernel multiplies f16 operands exactly and accumulates in f32 on the tensor core, so the only
@@ -45,7 +45,7 @@ CASES = [
 
 
 CASES_V2 = [(w, M, N, K, BN, f | 4) for (w, M, N, K, BN, f) in CASES] + [
-    (Q5_0, 1280, 6000, 1280, 256, 4),      # 10 x 24 = 240 tiles on 148 persistent CTAs: several tiles per CTA, both accumulators in use
+    (Q5_0, 1280, 6000, 1280, 256, 4),      # 10 x 24 = 240 tiles on 132 persistent CTAs: several tiles per CTA
     (Q5_0, 2560, 3000, 1280, 256, 5),
     (F16,  640,  4500, 320,  128, 4),
 ]

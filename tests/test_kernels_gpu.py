@@ -184,7 +184,7 @@ def test_encoder_flash_attention_kernel(lib):
 
 def test_whisper_bench_entry_points_measure_the_device(lib):
     """whisper_bench_memcpy_str / whisper_bench_ggml_mul_mat_str (whisper.h:746-753, `whisper-bench -w 1|2`) report device copy bandwidth
-    and tcgen05 GEMM throughput"""
+    and wgmma GEMM throughput"""
     import ctypes as C
     import re
     lib.whisper_bench_memcpy_str.restype = C.c_char_p; lib.whisper_bench_ggml_mul_mat_str.restype = C.c_char_p

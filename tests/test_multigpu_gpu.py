@@ -23,7 +23,7 @@ def _n_gpus():
         return 0
 
 
-@pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs (run under gpurun --gpus 2)")
+@pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs")
 def test_states_spread_over_gpus_and_results_match_single_gpu(lib, tmp_path):
     path = str(tmp_path / "m.bin")
     synth.write_model(path, "test-2l.en", Q5_0, seed=5, vocab_from=os.path.join(DATA_DIR, "for-tests-ggml-tiny.en.bin"))

@@ -33,7 +33,7 @@ def test_concurrent_callers_on_the_scripted_pool(lib, tmp_path):
     L = bind_whisper_api(lib)
     L.whisper_log_set.argtypes = [LOG_CB, vp]; L.whisper_log_set(_quiet, None)
     L.wb200_dbg_scripted_context.restype = vp; L.wb200_dbg_scripted_context.argtypes = [C.c_char_p]
-    en, _ = make_models(tmp_path)
+    en, _ = make_models(tmp_path, multilingual=False)
     ctx = L.wb200_dbg_scripted_context(en.encode())
     assert ctx
     n = 10

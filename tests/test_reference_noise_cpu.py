@@ -8,7 +8,7 @@ The unmodified reference CPU build gives different numbers for the same model an
     re-quantised to int8 blocks in front of every matrix (a rounding flip is a 1/127 step of the block maximum).
 This test measures that self-distance (1 thread vs 4 threads) on the synthetic 2-layer model and asserts it is what DESIGN.md quotes:
 logits 2e-2 .. 8e-2 of their standard deviation, i.e. as large as or larger than the distance between this engine and the 4-thread
-reference (tests/test_e2e_gpu.py: 2e-3 F16, 1.4e-2 Q5_0 measured on B200).  "Identical to the reference" can therefore only mean
+reference (tests/test_e2e_gpu.py holds the bounds per weight format).  "Identical to the reference" can therefore only mean
 "within the reference's own reproducibility", except where the arithmetic is integer or thread-independent (tokenizer, filters,
 samplers, KV bookkeeping, seek loop: pinned exactly elsewhere), or on a conditioned model (tests/test_exact_tokens_gpu.py).
 """

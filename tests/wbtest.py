@@ -82,7 +82,29 @@ def read_wav_f32(path):
     return (data.astype(np.float32) / 32768.0).astype(np.float32)
 
 
-DATA_DIR = os.path.join(ROOT, "oracle", "_ref", "data")
+DATA_DIR = os.path.join(ROOT, "oracle", "_ref", "data")          # data fixtures of the reference tree (make -C oracle data)
+
+
+def _stored_data_dir():
+    """Without the reference tree: the weight-less tiny.en model file of the reference's tests (header, mel filters, vocabulary), stored
+    compressed under tests/golden and unpacked once per user into the temporary directory."""
+    import lzma
+    import tempfile
+    d = os.path.join(tempfile.gettempdir(), "wb200-test-data-%d" % os.getuid())
+    name = "for-tests-ggml-tiny.en.bin"
+    if not os.path.exists(os.path.join(d, name)):
+        os.makedirs(d, exist_ok=True)
+        with lzma.open(os.path.join(ROOT, "tests", "golden", name + ".xz")) as f:
+            data = f.read()
+        tmp = os.path.join(d, "%s.%d" % (name, os.getpid()))
+        with open(tmp, "wb") as f:
+            f.write(data)
+        os.replace(tmp, os.path.join(d, name))
+    return d
+
+
+if not os.path.exists(os.path.join(DATA_DIR, "for-tests-ggml-tiny.en.bin")):
+    DATA_DIR = _stored_data_dir()
 
 
 def parse_model_header(path):

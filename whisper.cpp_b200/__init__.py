@@ -1,4 +1,4 @@
-"""whisper.cpp_b200 -- B200-native (sm_100a) Whisper inference engine behind the whisper.h C ABI.
+"""whisper.cpp_b200 -- CUDA-native Whisper inference engine for the H100 (sm_90a), behind the whisper.h C ABI.
 
 The product is `libwhisper_b200.so` (CUDA + C++, built in-tree by `make -C whisper.cpp_b200`).  This package only
 holds the host-side Python mirror of the reference interface (`api.py`) and the synthetic-model tooling (`synth.py`).

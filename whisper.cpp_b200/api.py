@@ -141,7 +141,7 @@ class WhisperB200:
 
     def __init__(self, model_path, gpu_device=0, lib_path=LIB_PATH):
         if not os.path.exists(lib_path):
-            raise RuntimeError(f"{lib_path} is missing: build it with __graft_entry__.build() (nvcc, sm_100a); there is no CPU fallback")
+            raise RuntimeError(f"{lib_path} is missing: build it with __graft_entry__.build() (nvcc, sm_90a); there is no CPU fallback")
         self.L = bind_whisper_api(C.CDLL(lib_path))
         self.L.wb200_last_error.restype = C.c_char_p
         self.L.wb200_launch_count.restype = C.c_uint64

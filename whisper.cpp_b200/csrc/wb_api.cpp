@@ -543,7 +543,7 @@ WB_EXPORT struct whisper_context * whisper_init_with_params_no_state(struct whis
     bool ok = false;
     try {
         if (!params.use_gpu) {
-            set_error("this engine runs on a B200 only: whisper_context_params.use_gpu=false is not supported (no CPU fallback)");
+            set_error("this engine runs on the GPU only: whisper_context_params.use_gpu=false is not supported (no CPU fallback)");
         } else {
             int ndev = 0;
             if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
@@ -888,7 +888,7 @@ WB_EXPORT void whisper_reset_timings(struct whisper_context * ctx) {
 }
 WB_EXPORT const char * whisper_print_system_info(void) {
     static std::string s;
-    s = "WHISPER_B200 : CUDA = 1 | ARCH = sm_100a | TCGEN05 = 1 | TMA = 1 | CPU_FALLBACK = 0 | ";
+    s = "WHISPER_B200 : CUDA = 1 | ARCH = sm_90a | WGMMA = 1 | TMA = 1 | CPU_FALLBACK = 0 | ";
     int ndev = 0; if (cudaGetDeviceCount(&ndev) == cudaSuccess) s += "DEVICES = " + std::to_string(ndev) + " | ";
     return s.c_str();
 }
@@ -896,7 +896,7 @@ WB_EXPORT void whisper_log_set(ggml_log_callback cb, void * user_data) {
     set_log_sink(reinterpret_cast<void (*)(int, const char *, void *)>(cb), user_data);
 }
 // whisper_bench_memcpy / whisper_bench_ggml_mul_mat (whisper.h:746-753; `whisper-bench -w 1|2`): the reference measures its CPU backend's
-// memcpy and ggml_mul_mat; here the same entry points measure what this engine runs on -- device copy bandwidth and the tcgen05 GEMM.
+// memcpy and ggml_mul_mat; here the same entry points measure what this engine runs on -- device copy bandwidth and the wgmma GEMM.
 static std::string bench_memcpy_str() {
     std::string out;
     char line[256];
@@ -925,7 +925,7 @@ static std::string bench_memcpy_str() {
 static std::string bench_mul_mat_str() {
     std::string out;
     char line[256];
-    out += "tcgen05 GEMM, f16 x f16 -> f32 (persistent kernel, wb_gemm.cu); C[N][M] = A[M][K] . B[N][K]^T\n";
+    out += "wgmma GEMM, f16 x f16 -> f32 (persistent kernel, wb_gemm.cu); C[N][M] = A[M][K] . B[N][K]^T\n";
     const int sizes[] = { 256, 512, 1024, 2048, 4096, 8192 };
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int n : sizes) {

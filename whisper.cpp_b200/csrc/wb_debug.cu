@@ -12,8 +12,8 @@ extern "C" {
 
 // C[n][m] (f32, token-major) = sum_k W[m][k] * X[n][k] ; W given in FILE layout (f16 rows or ggml quant blocks),
 // X given as f32 and rounded to f16 on the way in (as the engine does).  flags bit0: apply gelu; bit1: m-major output;
-// bit2: the persistent double-buffered kernel (quantised weights expanded to f16 once, both operands through TMA); bit3 (with bit2):
-// CTA pairs sharing the activation tile by TMA multicast, bit4 = f16 output, bit5 = in-place f32 residual (out holds x on entry).
+// bit2: the persistent kernel (quantised weights expanded to f16 once, both operands through TMA); bit3: the activation tile fetched
+// as two half-height TMA boxes, bit4 = f16 output, bit5 = in-place f32 residual (out holds x on entry).
 __attribute__((visibility("default")))
 int wb200_dbg_gemm(int wtype, int M, int N, int K, const void * w_file, const float * x, const float * bias,
                    float * out, int BN, int flags) {
@@ -39,7 +39,7 @@ int wb200_dbg_gemm(int wtype, int M, int N, int K, const void * w_file, const fl
         g.A.type = wtype; g.A.N = M; g.A.K = K; g.A.base = wraw.p;
     } else { set_error("wb200_dbg_gemm: unsupported wtype %d", wtype); return -5; }
     if (!make_tmap_f16(&g.tmB, xh.p, K, N, 1, 1, K, 0, 0, (flags & 8) ? BN / 2 : BN)) return -3;
-    if (flags & 8) g.cluster2 = 1;
+    if (flags & 8) g.half_box_b = 1;
     DevBuf<__half> a16;
     if (flags & 4) {
         g.v2 = 1;

@@ -17,7 +17,7 @@
 //     16 sectors per 128 useful bytes and the phase was L1-sector bound;
 //   * cross-attention (the HBM-heavy part: 2*n_keys*d f16 per row and layer) is cut into (row, head, half of the keys) units,
 //     streamed through a cp.async ring; one lane owns one key-quarter and keeps its own online-softmax state.
-// Lessons that shaped the code (profiles/): no pointers handed through structs (they turn shared-memory accesses into generic
+// Lessons that shaped the code: no pointers handed through structs (they turn shared-memory accesses into generic
 // loads), no 64-bit divisions in loops, approximate reciprocals where they only feed a rounding, no register moves of
 // in-flight loads, whole 32-byte sectors per load instruction, bulk copies instead of register staging for anything > 16 KB.
 #include <cmath>

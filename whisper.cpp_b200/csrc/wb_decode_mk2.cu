@@ -2,7 +2,7 @@
 //
 // What it computes is whisper_build_graph_decoder (src/whisper.cpp:2466-2844) for the rows of one whisper_batch (<= 64 rows).
 //
-// Why a second generation: in the first one all 148 CTAs walk the same phase together.  Per layer that is ~160 us of latency-bound
+// Why a second generation: in the first one all CTAs (one per SM) walk the same phase together.  Per layer that is ~160 us of latency-bound
 // phases (GEMV of a few MB, LayerNorm, self-attention, 11 grid barriers) that leave HBM idle, followed by ~100 us of cross-attention
 // that is purely HBM-bound (503 MB of cross K/V per layer at 64 rows = 90 % of the bytes of the pass).  The two kinds of work never
 // overlap, so the pass sits at 0.31 of the HBM roofline although the streaming part alone runs at 0.8.

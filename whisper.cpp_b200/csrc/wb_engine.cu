@@ -1,6 +1,6 @@
 // wb_engine.cu -- see wb_engine.h.  Graph structure follows whisper_build_graph_conv / _encoder / _cross / _decoder
 // (src/whisper.cpp:1982-2042, 2044-2275, 2278-2354, 2466-2844); every `ggml_mul_mat (+add/scale/gelu/cpy)` group of the
-// reference is one tcgen05 GEMM launch (encode) or one fused GEMV launch (decode step) here.
+// reference is one wgmma GEMM launch (encode) or one fused GEMV launch (decode step) here.
 #include <algorithm>
 #include <cmath>
 #include <chrono>
@@ -51,7 +51,6 @@ bool Engine::init(const Model * model, int cap_windows) {
     use_graphs = getenv("WB200_NO_GRAPHS") == nullptr;
     fused_attn = getenv("WB200_UNFUSED_ATTN") == nullptr;
     gemm_v2 = getenv("WB200_GEMM_V1") == nullptr;
-    gemm_cluster = !(getenv("WB200_GEMM_CLUSTER") && atoi(getenv("WB200_GEMM_CLUSTER")) == 0);
     if (gemm_v2 && m->wtype != WT_F16 && m->wtype != WT_F32 && !m->cross_kv.f16) {
         const size_t dd = (size_t) hp.n_audio_state * hp.n_audio_state;
         if (!wf16.alloc(std::max<size_t>(4 * dd, (size_t) 2 * hp.n_text_layer * dd))) return false;
@@ -69,7 +68,7 @@ bool Engine::init(const Model * model, int cap_windows) {
         }
         if (const char * pf = getenv("WB200_MK_PREFETCH")) mk_prefetch = atoi(pf);
         // WB200_MK_GEN=2 selects the experimental second generation (row groups walking the layers independently, two CTAs per SM):
-        // measured slower (10.1 ms against 8.6 ms per 64-row pass, profiles/r02_mk2_experiment.md), kept for the A/B
+        // slower than the first generation where it was measured (DESIGN.md section 4), kept for the A/B
         mk_gen = 1;
         if (const char * ge = getenv("WB200_MK_GEN")) mk_gen = atoi(ge) == 2 ? 2 : 1;
         if (use_mk && mk_gen == 2 && !mk2_supported(m->wtype == WT_F32 ? WT_F16 : m->wtype, hp.n_text_state)) mk_gen = 1;
@@ -313,19 +312,16 @@ static bool build_plan(Engine & E, int n_ctx, int n_win) {
     }
     // activation-side tile: 256 tokens per CTA, or 128 when a d x NT GEMM would otherwise leave SMs idle (one window: 10 x 6 = 60 CTAs)
     const int bn = (((NT + 255) / 256) * ((d + 127) / 128) < E.n_sm) ? 128 : 256;
-    // CTA pairs share the activation tile by TMA multicast (gemm2_kernel<BN, 2>): each CTA of a pair fetches half of it, so the box is bn / 2 rows
-    const bool cl2 = E.gemm_v2 && E.gemm_cluster && (E.wf16.p || m.cross_kv.f16 || m.wtype == WT_F16 || m.wtype == WT_F32);
-    const int bbox = cl2 ? bn / 2 : bn;
     CUtensorMap tm_xn, tm_xn_win, tm_attn, tm_hfc, tm_q, tm_k, tm_p, tm_vt, tm_enc;
-    if (!make_tmap_f16(&tm_xn, E.xn.p, d, NT, 1, 1, d, 0, 0, bbox)) return false;
-    if (!make_tmap_f16(&tm_xn_win, E.xn.p, d, T, n_win, 1, d, (uint64_t) T * d, 0, bbox)) return false;
-    if (!make_tmap_f16(&tm_attn, E.attn.p, d, NT, 1, 1, d, 0, 0, bbox)) return false;
-    if (!make_tmap_f16(&tm_hfc, E.hfc.p, 4*d, NT, 1, 1, 4*d, 0, 0, bbox)) return false;
+    if (!make_tmap_f16(&tm_xn, E.xn.p, d, NT, 1, 1, d, 0, 0, bn)) return false;
+    if (!make_tmap_f16(&tm_xn_win, E.xn.p, d, T, n_win, 1, d, (uint64_t) T * d, 0, bn)) return false;
+    if (!make_tmap_f16(&tm_attn, E.attn.p, d, NT, 1, 1, d, 0, 0, bn)) return false;
+    if (!make_tmap_f16(&tm_hfc, E.hfc.p, 4*d, NT, 1, 1, 4*d, 0, 0, bn)) return false;
     if (!make_tmap_f16(&tm_q, E.qk.p,     64, T, H, n_win, 2*d, 64, (uint64_t) T * 2 * d, 256)) return false;
     if (!make_tmap_f16(&tm_k, E.qk.p + d, 64, T, H, n_win, 2*d, 64, (uint64_t) T * 2 * d, 128)) return false;
     if (!E.fused_attn && !make_tmap_f16(&tm_p, E.P.p, Tp, T, H, n_win, Tp, (uint64_t) T * Tp, (uint64_t) H * T * Tp, 128)) return false;
     if (!make_tmap_f16(&tm_vt, E.vt.p, Tp, 64, H, n_win, Tp, (uint64_t) 64 * Tp, (uint64_t) d * Tp, 64)) return false;
-    if (!make_tmap_f16(&tm_enc, E.enc16.p, d, T, n_win, 1, d, (uint64_t) T * d, 0, bbox)) return false;
+    if (!make_tmap_f16(&tm_enc, E.enc16.p, d, T, n_win, 1, d, (uint64_t) T * d, 0, bn)) return false;
 
     P.layers.resize(La);
     for (int l = 0; l < La; ++l) {
@@ -379,10 +375,8 @@ static bool build_plan(Engine & E, int n_ctx, int n_win) {
         if (!to_v2(P.conv1, 0) || !to_v2(P.conv2, 0) || !to_v2(P.conv2_tap, 0)) return false;
         for (auto & lp : P.layers) {
             if (!to_v2(lp.qk, 2*d) || !to_v2(lp.v, d) || !to_v2(lp.o, d) || !to_v2(lp.fc1, 4*d) || !to_v2(lp.fc2, d)) return false;
-            for (GemmDesc * g : { &lp.qk, &lp.v, &lp.o, &lp.fc1, &lp.fc2 }) g->cluster2 = (cl2 && g->v2) ? 1 : 0;
         }
         if (!to_v2(P.cross, (int64_t) 2 * Lt * d)) return false;
-        P.cross.cluster2 = (cl2 && P.cross.v2) ? 1 : 0;
     }
     return true;
 }

@@ -56,7 +56,6 @@ struct Engine {
     DevBuf<__half> mel_win, h1, xn, qk, vt, P, attn, hfc, enc16;
     DevBuf<float>  x, S, enc32, conv32;
     DevBuf<__half> wf16;             // f16 expansion of the quantised matrix the current encoder GEMM multiplies (wb_gemm.cu, k_dequant_f16)
-    bool gemm_cluster = true;        // WB200_GEMM_CLUSTER=0: no CTA pairs / TMA multicast in the persistent GEMM
     bool gemm_v2 = true;             // WB200_GEMM_V1=1 selects the first-generation kernel (in-kernel dequantisation, one tile per CTA)
     DevBuf<__half> kv_cross;         // [cap_win][2][Lt][Tp][d]; with the persistent decode kernel (use_mk) each [Tp][d] block is head-major [d/64][Tp][64]
     int enc_n_ctx = 0, enc_n_win = 0;   // what the last encode produced

@@ -1,4 +1,4 @@
-// wb_fattn.cu -- fused encoder self-attention on tcgen05 (replaces ggml_flash_attn_ext in whisper_build_graph_encoder,
+// wb_fattn.cu -- fused encoder self-attention on wgmma (replaces ggml_flash_attn_ext in whisper_build_graph_encoder,
 // src/whisper.cpp:2142-2167; CPU semantics ggml/src/ggml-cpu/ops.cpp:8479-8715).
 //
 //   out[q, h*64 + :] = softmax_k( scale * Q_h[q,:] . K_h[k,:] ) @ V_h[k,:]     over k = 0 .. 1535
@@ -7,19 +7,13 @@
 // n_ctx are zero-filled by TMA and the V^T buffer keeps zeros in those columns, so they take part in max and sum exactly
 // like in the reference.
 //
-// One CTA = 128 queries (TMEM lanes) of one head.  Two passes over the 24 key blocks of 64:
-//   pass 1  S_j = Q K_j^T (4 x tcgen05.mma M128 N64 K16)  -> row maxima only
-//   pass 2  S_j again, p = exp2((s - m) * scale*log2e) with the FINAL maximum m, P_j -> smem (f16, swizzled K-major),
-//           O += P_j V_j (4 x tcgen05.mma M128 N64 K16) accumulated in TMEM, l += sum p
-// TWO CTAs share an SM (88 KB of shared memory and 256 tensor-memory columns each; blocks of 64 keys make that fit): the kernel is
-// bound by the softmax warps -- 16 ex2 per clock per SM, and chains of TMEM load -> exponent -> smem store -> mbarrier -- and a single
-// CTA per SM left the exponent pipe idle during its first pass, its prologue and its epilogue (measured: 20 us per CTA against 6.4 us
-// of ex2 work).
-// Knowing m before any exponent is taken removes the online-softmax rescaling of O (no TMEM read-modify-write, no
-// correction warps); the price is recomputing QK^T once: +1/3 tensor work on 14% of the encoder flops.
-// Roles: warp 0 TMA producer, warp 1 MMA issuer (one thread), warps 2..9 softmax + epilogue: a query row is shared by two threads (TMEM
-// lane quarter = warp % 4), each takes 64 of the 128 keys of a block -- the phase is bound by the 16 ex2 per clock of the SM, and four
-// warps alone could not keep that pipe busy across the TMEM-load / barrier latencies.
+// One CTA = 128 queries of one head, three warpgroups: warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 own 64 queries
+// each.  Two passes over the 24 key blocks of 64:
+//   pass 1  S_j = Q K_j^T (4 x wgmma m64n64k16, both operands in smem, S in registers)  -> row maxima only
+//   pass 2  S_j again, p = exp2((s - m) * scale*log2e) with the FINAL maximum m, rounded to f16 in registers, which are the A operand of
+//           O += P_j V_j (4 x wgmma m64n64k16, A from registers, V^T from smem) accumulated in registers, l += sum p
+// Knowing m before any exponent is taken removes the online-softmax rescaling of O; the price is recomputing QK^T once: +1/3 tensor work
+// on 14% of the encoder flops.
 #include "wb_gemm.cuh"
 #include "wb_ptx.cuh"
 #include "wb_common.h"
@@ -27,17 +21,18 @@
 
 namespace wb {
 
-static constexpr int FA_THREADS = 320;
+static constexpr int FA_THREADS = 384;
 static constexpr int FA_KSTAGES = 3, FA_VSTAGES = 2;
 static constexpr int FA_KB = 64;                   // keys per block
-static constexpr int FA_Q_BYTES = 128 * 128, FA_K_BYTES = FA_KB * 128, FA_V_BYTES = 64 * FA_KB * 2, FA_P_BYTES = 128 * FA_KB * 2;
-static constexpr int FA_SMEM = FA_Q_BYTES + FA_KSTAGES * FA_K_BYTES + FA_VSTAGES * FA_V_BYTES + 2 * FA_P_BYTES + 1024 + 256 + 2 * 128 * 4;
+static constexpr int FA_Q_BYTES = 128 * 128, FA_K_BYTES = FA_KB * 128, FA_V_BYTES = 64 * FA_KB * 2;
+static constexpr int FA_SMEM = FA_Q_BYTES + FA_KSTAGES * FA_K_BYTES + FA_VSTAGES * FA_V_BYTES + 1024 + 256;
 
 struct FattnParams { int T, n_kb; float scale_log2e; __half * out; int64_t ldo, out_win; };
 
 __device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t *>(&h); }
 
-__global__ void __launch_bounds__(FA_THREADS, 2)
+__global__ void __launch_bounds__(FA_THREADS, 1)
 fattn_enc_kernel(const FattnParams p, const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV) {
     extern __shared__ uint8_t smem_raw[];
@@ -45,39 +40,27 @@ fattn_enc_kernel(const FattnParams p, const __grid_constant__ CUtensorMap tmQ, c
     uint8_t * sQ = smem;
     uint8_t * sK = sQ + FA_Q_BYTES;
     uint8_t * sV = sK + FA_KSTAGES * FA_K_BYTES;
-    uint8_t * sP = sV + FA_VSTAGES * FA_V_BYTES;
-    uint64_t * bars = reinterpret_cast<uint64_t *>(sP + 2 * FA_P_BYTES);
+    uint64_t * bars = reinterpret_cast<uint64_t *>(sV + FA_VSTAGES * FA_V_BYTES);
     uint64_t * k_full = bars,       * k_empty = bars + 3;
     uint64_t * v_full = bars + 6,   * v_empty = bars + 8;
-    uint64_t * s_full = bars + 10,  * s_free  = bars + 12;
-    uint64_t * p_full = bars + 14,  * p_free  = bars + 16;
-    uint64_t * q_full = bars + 18,  * o_full  = bars + 19;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 20);
-    float * xch = reinterpret_cast<float *>(bars + 32);          // [2][128]: row maxima / row sums of the two column halves
+    uint64_t * q_full = bars + 10;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * 128, h = blockIdx.y, w = blockIdx.z;
     const int n_kb = p.n_kb;
 
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < FA_KSTAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1); }
-        for (int i = 0; i < FA_VSTAGES; ++i) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_free[i], 8); mbar_init(&p_full[i], 8); mbar_init(&p_free[i], 1); }
-        mbar_init(q_full, 1); mbar_init(o_full, 1);
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
+        for (int i = 0; i < FA_KSTAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 8); }    // released by the 8 MMA warps
+        for (int i = 0; i < FA_VSTAGES; ++i) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 8); }
+        mbar_init(q_full, 1);
         mbar_fence_init();
     }
-    if (warp == 2) tmem_alloc<256>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tS[2] = { tmem, tmem + FA_KB };
-    const uint32_t tO = tmem + 2 * FA_KB;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ---------------------------------------------------------------- TMA producer
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             mbar_arrive_expect_tx(q_full, FA_Q_BYTES);
             tma_load_4d(sQ, &tmQ, q_full, 0, q0, h, w);
             int ks = 0; uint32_t kph = 0; int vs = 0; uint32_t vph = 0;
@@ -96,148 +79,86 @@ fattn_enc_kernel(const FattnParams p, const __grid_constant__ CUtensorMap tmQ, c
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------------------------------------------------------- MMA issuer
-        if (lane == 0) {
-            const uint32_t id_qk = umma_idesc_f16(128, FA_KB), id_pv = umma_idesc_f16(128, 64);
-            const uint64_t qdesc = umma_desc_sw128(smem_u32(sQ));
-            mbar_wait(q_full, 0);
-            int ks = 0; uint32_t kph = 0; int vs = 0; uint32_t vph = 0;
-            uint32_t sfree_ph[2] = { 0, 0 }, pfull_ph[2] = { 0, 0 };
-            int it = 0;                                   // global S-buffer use counter
-            auto issue_pv = [&](int jb) {                 // O += P[jb&1] * V
-                const int b = jb & 1;
-                mbar_wait(&p_full[b], pfull_ph[b]); pfull_ph[b] ^= 1;
-                mbar_wait(&v_full[vs], vph);
-                tc_fence_after();
-                const uint32_t pbase = smem_u32(sP + b * FA_P_BYTES), vbase = smem_u32(sV + vs * FA_V_BYTES);
-#pragma unroll
-                for (int s = 0; s < FA_KB / 16; ++s) {
-                    const uint64_t ad = umma_desc_sw128(pbase + s * 32);
-                    const uint64_t bd = umma_desc_sw128(vbase + s * 32);
-                    umma_f16_ss(tO, ad, bd, id_pv, (jb | s) ? 1u : 0u);
-                }
-                umma_commit(&p_free[b]);
-                umma_commit(&v_empty[vs]);
-                if (++vs == FA_VSTAGES) { vs = 0; vph ^= 1; }
-            };
-            for (int pass = 0; pass < 2; ++pass) {
-                for (int j = 0; j < n_kb; ++j, ++it) {
-                    const int b = it & 1;
-                    mbar_wait(&k_full[ks], kph);
-                    if (it >= 2) { mbar_wait(&s_free[b], sfree_ph[b]); sfree_ph[b] ^= 1; }
-                    tc_fence_after();
-                    const uint64_t kdesc = umma_desc_sw128(smem_u32(sK + ks * FA_K_BYTES));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ss(tS[b], qdesc + 2*k, kdesc + 2*k, id_qk, k ? 1u : 0u);
-                    umma_commit(&s_full[b]);
-                    umma_commit(&k_empty[ks]);
-                    if (++ks == FA_KSTAGES) { ks = 0; kph ^= 1; }
-                    if (pass == 1 && j > 0) issue_pv(j - 1);
-                }
-            }
-            issue_pv(n_kb - 1);
-            umma_commit(o_full);
-        }
-    } else {
-        // ---------------------------------------------------------------- softmax warps (thread = query row) + epilogue
-        const int q = warp & 3;                            // TMEM lane quarter of this warp
-        const int half = (warp - 2) >> 2;                  // which 32 keys of a block (pass 1, 2) / which 32 output dims (epilogue)
-        const int row = q * 32 + lane;                     // query row inside the tile
-        const uint32_t lane_off = (uint32_t) (q * 32) << 16;
-        uint32_t sfull_ph[2] = { 0, 0 }, pfree_ph[2] = { 0, 0 };
-        float m = -INFINITY;
-        int it = 0;
-        // pass 1: row maximum of the raw scores
-        for (int j = 0; j < n_kb; ++j, ++it) {
-            const int b = it & 1;
-            mbar_wait(&s_full[b], sfull_ph[b]); sfull_ph[b] ^= 1;
-            tc_fence_after();
-            {
-                uint32_t v[32];
-                tmem_ld_32x32(tS[b] + lane_off + half * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) m = fmaxf(m, __uint_as_float(v[i]));
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_free[b]);
-        }
-        xch[half * 128 + row] = m;
-        bar_named(1, 256);
-        m = fmaxf(m, xch[(half ^ 1) * 128 + row]);
-        const float mc = m * p.scale_log2e;
-        float l = 0.0f;
-        const int sw = row & 7;
-        // pass 2: probabilities with the final maximum; P -> smem (two 64-key swizzle atoms), l += sum p
-        for (int j = 0; j < n_kb; ++j, ++it) {
-            const int b = it & 1;
-            mbar_wait(&s_full[b], sfull_ph[b]); sfull_ph[b] ^= 1;
-            if (j >= 2) { mbar_wait(&p_free[b], pfree_ph[b]); pfree_ph[b] ^= 1; }
-            tc_fence_after();
-            uint8_t * prow = sP + b * FA_P_BYTES + row * 128;
-            {
-                const int c = half;
-                uint32_t v[32];
-                tmem_ld_32x32(tS[b] + lane_off + c * 32, v);
-                tmem_ld_wait();
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float p0 = ex2f(fmaf(__uint_as_float(v[2*i]),     p.scale_log2e, -mc));
-                    const float p1 = ex2f(fmaf(__uint_as_float(v[2*i + 1]), p.scale_log2e, -mc));
-                    const __half2 hp = __floats2half2_rn(p0, p1);
-                    // the tensor core consumes the ROUNDED probabilities: accumulate the same values into the denominator
-                    const float2 pr = __half22float2(hp);
-                    l += pr.x + pr.y;
-                    pk[i] = *reinterpret_cast<const uint32_t *>(&hp);
-                }
-                // keys c*32 .. c*32+31 of this block: 16-byte chunks c*4 .. +3 of the 128-byte row (one swizzle atom)
-                uint8_t * arow = prow;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int chunk = c * 4 + u;
-                    *reinterpret_cast<uint4 *>(arow + ((chunk ^ sw) << 4)) = make_uint4(pk[4*u], pk[4*u + 1], pk[4*u + 2], pk[4*u + 3]);
-                }
-            }
-            fence_proxy_async_smem();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(&s_free[b]); mbar_arrive(&p_full[b]); }
-        }
-        // epilogue: O / l -> f16 -> global
-        bar_named(1, 256);                                 // everybody has read the maxima
-        xch[half * 128 + row] = l;
-        bar_named(1, 256);
-        l = xch[row] + xch[128 + row];                     // fixed order: both threads of a row get the same sum
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        const int qg = q0 + row;
-        const float inv = 1.0f / l;
-        __half * orow = p.out + (int64_t) w * p.out_win + (int64_t) qg * p.ldo + h * 64;
-        {
-            const int c = half;
-            uint32_t v[32];
-            tmem_ld_32x32(tO + lane_off + c * 32, v);
-            tmem_ld_wait();
-            if (qg < p.T) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 8) {
-                    uint32_t o[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const __half2 hh = __floats2half2_rn(__uint_as_float(v[i + 2*e]) * inv, __uint_as_float(v[i + 2*e + 1]) * inv);
-                        o[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                    }
-                    *reinterpret_cast<uint4 *>(orow + c * 32 + i) = make_uint4(o[0], o[1], o[2], o[3]);
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc<256>(tmem);
+
+    // -------------------------------------------------------------------- MMA + softmax warpgroups
+    // thread t holds query rows r0 = 16*(t/32) + (t%32)/4 and r0 + 8 of its warpgroup's 64, key / output columns 8*j + 2*(t%4) (+1)
+    const int cw = wg - 1, t = threadIdx.x & 127;
+    const int r0 = cw * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+    const uint64_t qdesc = wgmma_desc_sw128(smem_u32(sQ + cw * 64 * 128));
+    int ks = 0; uint32_t kph = 0;
+    float S[32];
+    auto scores = [&]() {                                  // S = Q K_j^T of the next K stage; the stage is released afterwards
+        mbar_wait(&k_full[ks], kph);
+        wgmma_fence();
+        const uint64_t kdesc = wgmma_desc_sw128(smem_u32(sK + ks * FA_K_BYTES));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_f16_ss<64>(S, qdesc + 2*k, kdesc + 2*k, k ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(S);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&k_empty[ks]);
+        if (++ks == FA_KSTAGES) { ks = 0; kph ^= 1; }
+    };
+    mbar_wait(q_full, 0);
+    // pass 1: row maxima of the raw scores
+    float m[2] = { -INFINITY, -INFINITY };
+    for (int j = 0; j < n_kb; ++j) {
+        scores();
+#pragma unroll
+        for (int i = 0; i < 32; ++i) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], S[i]);
+    }
+    float mc[2], l[2] = { 0.0f, 0.0f };
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
+        mc[r] = m[r] * p.scale_log2e;
+    }
+    // pass 2: probabilities with the final maximum, O += P V
+    float O[32];
+    int vs = 0; uint32_t vph = 0;
+    for (int j = 0; j < n_kb; ++j) {
+        scores();
+        uint32_t a[4][4];
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+            const int r = (i >> 1) & 1;
+            const float p0 = ex2f(fmaf(S[i],     p.scale_log2e, -mc[r]));
+            const float p1 = ex2f(fmaf(S[i + 1], p.scale_log2e, -mc[r]));
+            const uint32_t hp = pack_half2(p0, p1);
+            // the tensor core consumes the ROUNDED probabilities: accumulate the same values into the denominator
+            const float2 pr = __half22float2(*reinterpret_cast<const __half2 *>(&hp));
+            l[r] += pr.x + pr.y;
+            a[i >> 3][(i & 7) >> 1] = hp;                  // keys 16*s .. 16*s + 15 = S[8s .. 8s + 7]: the A fragment of k-step s
+        }
+        mbar_wait(&v_full[vs], vph);
+        wgmma_fence();
+        const uint64_t vdesc = wgmma_desc_sw128(smem_u32(sV + vs * FA_V_BYTES));
+#pragma unroll
+        for (int s = 0; s < 4; ++s) wgmma_f16_rs_n64(O, a[s], vdesc + 2*s, (j | s) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(O);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&v_empty[vs]);
+        if (++vs == FA_VSTAGES) { vs = 0; vph ^= 1; }
+    }
+    // epilogue: O / l -> f16 -> global
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+        const int qg = q0 + r0 + 8 * r;
+        if (qg >= p.T) continue;
+        const float inv = 1.0f / l[r];
+        __half * orow = p.out + (int64_t) w * p.out_win + (int64_t) qg * p.ldo + h * 64 + 2 * (t & 3);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+            *reinterpret_cast<uint32_t *>(orow + 8 * jj) = pack_half2(O[4 * jj + 2 * r] * inv, O[4 * jj + 2 * r + 1] * inv);
+    }
 }
 
 // Q, K: f16 [n_win][T][ld_qk] with head h at columns h*64 (K at +k_off); Vt: f16 [n_win][H*64][Tp]; out: f16 [n_win*T][ldo]

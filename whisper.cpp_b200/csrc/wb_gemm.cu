@@ -1,15 +1,19 @@
-// wb_gemm.cu -- the tcgen05 GEMM used by every dense contraction of the encode path
+// wb_gemm.cu -- the wgmma GEMM used by every dense contraction of the encode path
 // (conv stem, encoder QKV/O/MLP, cross K/V, attention scores and PV in the unfused path, decoder prompt).
 //
-// One CTA computes a 128 (weight rows, TMEM lanes) x BN (activation rows, TMEM columns) tile:
-//   warp 0      : TMA producer   -- B tile (and A tile for f16 weights) into a STAGES-deep smem ring
-//   warp 1      : MMA issuer     -- one thread issues 4 x tcgen05.mma (K=16) per 64-wide k-block, commits to mbarriers
-//   warps 2..9  : quant decoders -- (quantised A only) each thread turns one 32-value block into 32 halves and
-//                                   stores them into the 128B-swizzled K-major operand tile;
-//                                   after the main loop the same warps run the epilogue (TMEM -> regs -> global)
-// Layout facts relied on (guides: blackwell_cuda_programming.md "UMMA", B300_MICROARCH.md "tcgen05"):
+// One CTA computes 128 (weight rows) x BN (activation rows) tiles, three warpgroups:
+//   warpgroup 0    : producer   -- thread 0 streams the B tile (and the A tile for f16 weights) into a STAGES-deep smem ring by TMA;
+//                                  for quantised A (first-generation launch) all 128 threads decode one weight row each (2 x 32-value
+//                                  blocks per 64-wide k-block) into the 128B-swizzled K-major operand tile
+//   warpgroups 1-2 : consumers  -- each owns 64 of the 128 weight rows: 4 x wgmma m64nBNk16 per k-block with the f32 accumulator in
+//                                  registers, then the epilogue (bias / scale / GELU / residual -> global) straight from those registers
+// The same kernel serves the first-generation launch (one tile per CTA, quantised weights decoded in the kernel) and the persistent one
+// (gridDim = number of SMs, each CTA walks the tile list, weight-tile index fastest so that concurrently running CTAs share activation
+// tiles in L2; quantised weights expanded to f16 beforehand by k_dequant_f16, both operands through TMA).  The producer runs ahead into the
+// next tile's k-blocks while the consumers run the epilogue of the current one.
+// Layout facts relied on:
 //   * K-major SW128 tile: row r at byte r*128, 16-byte chunk c stored at chunk (c ^ (r & 7)); 8-row groups 1024 B apart
-//   * a warp may only tcgen05.ld the TMEM lane quarter (warp_id % 4)
+//   * wgmma accumulator: thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8*j + 2*(t%4) (+1)
 #include <algorithm>
 #include "wb_gemm.cuh"
 #include "wb_ptx.cuh"
@@ -17,7 +21,7 @@
 
 namespace wb {
 
-static constexpr int GEMM_THREADS  = 320;
+static constexpr int GEMM_THREADS  = 384;
 static constexpr int A_TILE_BYTES  = 128 * 64 * 2;
 
 template <int BN> struct GemmCfg {
@@ -29,6 +33,8 @@ template <int BN> struct GemmCfg {
 struct GemmKParams {
     int M, N, K, taps, nkb_per_tap, nb0;
     int a_zsel0, a_zsel1, b_zsel0, b_zsel1, a_rows_per_b0, b1_in_off;
+    int n_mt, n_nt, n_tiles;        // tile list: weight tile fastest, then activation tile, then batch index
+    int b_split;                    // 2: the B tensor map's box holds BN / 2 rows (the tile is fetched in two halves)
     // quantised A
     const void * a_base; const uint8_t * a_qs; const uint32_t * a_qh; const __half * a_d;
     GemmEpilogue ep;
@@ -64,151 +70,56 @@ __device__ __forceinline__ void raw_load(const GemmKParams & p, int m, int k, Ra
     }
 }
 
-// Epilogue of one 128 x BN tile held in TMEM columns [tmem_acc, tmem_acc + BN): TMEM -> registers -> bias / scale / GELU / residual -> global.
-// Called by the 8 epilogue warps (warp = 2..9): warp & 3 selects the TMEM lane quarter the warp may read, (warp - 2) >> 2 the column half.
-template <int BN>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams & p, uint32_t tmem_base, int m0, int n0, int b0, int b1, int warp, int lane) {
-    const int q    = warp & 3;                 // TMEM lane quarter this warp may read
-    const int hsel = (warp - 2) >> 2;          // which half of the columns
-    const int m    = m0 + q * 32 + lane;
-    const bool mval = m < p.M;
-    const GemmEpilogue & e = p.ep;
-    const int mg = m + b0 * p.a_rows_per_b0;   // bias / scale follow the stacked-matrix row
-    const float bias = (mval && e.bias_m)  ? e.bias_m[mg]  : 0.0f;
-    const float scl  = ((mval && e.scale_m) ? e.scale_m[mg] : 1.0f) * e.alpha;
-    const int64_t ooff = (int64_t) b0 * e.out_b0 + (int64_t) b1 * e.out_b1;
-    const int64_t roff = (int64_t) b0 * e.res_b0 + (int64_t) b1 * e.res_b1;
-    constexpr int CH = BN / 2 / 32;            // 32-column chunks per warp
+// one accumulator value (weight row m, activation row n) through the epilogue; bias and scl belong to row m
+__device__ __forceinline__ void epilogue_elem(const GemmEpilogue & e, int64_t ooff, int64_t roff, int m, int n, float v, float bias, float scl) {
     if (e.res && !e.out_mmajor && !e.out_f16 && e.act == 0) {
-        // f32 residual stream (attention-O / FC2: x += W a): the residual values of chunk c+1 are requested before chunk c is drained, so
-        // a warp keeps two chunks (8 KB) in flight -- with one, the 128 KB of a tile took longer to arrive than its main loop runs
+        // f32 residual stream (attention-O / FC2: x += W a)
         float * o = reinterpret_cast<float *>(e.out) + ooff;
-        const float * rp = e.res + roff + m;
-        float rn[32];
-        auto fetch = [&](int col) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const int n = n0 + col + j;
-                rn[j] = (mval && n < p.N) ? __ldcg(rp + (int64_t) n * e.ldr) : 0.0f;
-            }
-        };
-        fetch(hsel * (BN / 2));
-        const float bs = bias * scl;
-#pragma unroll 1
-        for (int c = 0; c < CH; ++c) {
-            const int col = hsel * (BN / 2) + c * 32;
-            if (n0 + col >= p.N) break;        // warp-uniform
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) col, v);
-            float f[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = rn[j];
-            if (c + 1 < CH) fetch(col + 32);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const int n = n0 + col + j;
-                if (mval && n < p.N) o[(int64_t) (n + e.n_row_off) * e.ldo + m] = fmaf(__uint_as_float(v[j]), scl, bs) + f[j];
-            }
-        }
+        o[(int64_t) (n + e.n_row_off) * e.ldo + m] = fmaf(v, scl, bias * scl) + __ldcg(e.res + roff + (int64_t) n * e.ldr + m);
         return;
     }
     if (e.act == 1 && e.out_f16 && !e.res && !e.out_mmajor && e.hm_rows == 0) {
-        // FC1: GELU with the reference's f16 table semantics, a dozen instructions per value (the generic path below spends about twenty,
-        // which made this epilogue longer than the K = 1280 main loop): see gelu_ref_f16 for the formula and its accuracy
-        __half * o = reinterpret_cast<__half *>(e.out) + ooff;
-        const float bs = bias * scl;
-#pragma unroll 1
-        for (int c = 0; c < CH; ++c) {
-            const int col = hsel * (BN / 2) + c * 32;
-            if (n0 + col >= p.N) break;
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) col, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) {
-                const __half2 h2 = __floats2half2_rn(fmaf(__uint_as_float(v[j]), scl, bs), fmaf(__uint_as_float(v[j + 1]), scl, bs));
-                float2 x = __half22float2(h2);
-                x.x = fmaxf(x.x, -20.0f); x.y = fmaxf(x.y, -20.0f);            // gelu = 0 below -10 either way; keeps exp finite
-                const float e0 = __expf(x.x * fmaf(x.x * x.x, -0.07135481627f, -1.5957691216f));
-                const float e1 = __expf(x.y * fmaf(x.y * x.y, -0.07135481627f, -1.5957691216f));
-                const __half2 g2 = __floats2half2_rn(__fdividef(x.x, 1.0f + e0), __fdividef(x.y, 1.0f + e1));
-                const int n = n0 + col + j;
-                if (mval && n < p.N)     o[(int64_t) (n + e.n_row_off) * e.ldo + m]     = __low2half(g2);
-                if (mval && n + 1 < p.N) o[(int64_t) (n + 1 + e.n_row_off) * e.ldo + m] = __high2half(g2);
-            }
-        }
+        // FC1: GELU with the reference's f16 table semantics, a dozen instructions per value: see gelu_ref_f16 for the formula and its accuracy
+        float x = __half2float(__float2half_rn(fmaf(v, scl, bias * scl)));
+        x = fmaxf(x, -20.0f);                                           // gelu = 0 below -10 either way; keeps exp finite
+        const float ex = __expf(x * fmaf(x * x, -0.07135481627f, -1.5957691216f));
+        reinterpret_cast<__half *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = __float2half_rn(__fdividef(x, 1.0f + ex));
         return;
     }
-#pragma unroll 1
-    for (int c = 0; c < CH; ++c) {
-        const int col = hsel * (BN / 2) + c * 32;
-        if (n0 + col >= p.N) break;            // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) col, v);
-        tmem_ld_wait();
-        float f[32];
+    float x = (v + bias) * scl;
+    if (e.act == 1) x = gelu_ref_f16(x);
+    if (e.res) x += e.res[roff + (int64_t) n * e.ldr + m];
+    if (e.out_mmajor) {
+        if (e.out_f16) reinterpret_cast<__half *>(e.out)[ooff + (int64_t) m * e.ldo + n] = __float2half_rn(x);
+        else           reinterpret_cast<float *>(e.out)[ooff + (int64_t) m * e.ldo + n] = x;
+    } else if (e.out_f16 && e.hm_rows > 0) {                           // head-major: 64 consecutive features of a key are one 128-byte row
+        reinterpret_cast<__half *>(e.out)[ooff + (int64_t) (m >> 6) * e.hm_rows * 64 + (int64_t) (n + e.n_row_off) * 64 + (m & 63)] = __float2half_rn(x);
+    } else if (e.out_f16) {
+        reinterpret_cast<__half *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = __float2half_rn(x);
+    } else {
+        reinterpret_cast<float *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = x;
+    }
+}
+
+// epilogue of the 64 x BN accumulator of one consumer warpgroup (rows m0 .. m0 + 63 of the weight side, columns n0 .. n0 + BN - 1)
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_regs(const GemmKParams & p, const float (&acc)[BN / 2], int m0, int n0, int b0, int b1, int t) {
+    const GemmEpilogue & e = p.ep;
+    const int64_t ooff = (int64_t) b0 * e.out_b0 + (int64_t) b1 * e.out_b1;
+    const int64_t roff = (int64_t) b0 * e.res_b0 + (int64_t) b1 * e.res_b1;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            float x = (__uint_as_float(v[j]) + bias) * scl;
-            if (e.act == 1) x = gelu_ref_f16(x);
-            f[j] = x;
-        }
-        if (e.res) {
+    for (int h = 0; h < 2; ++h) {
+        const int m = m0 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;
+        if (m >= p.M) continue;
+        const int mg = m + b0 * p.a_rows_per_b0;                        // bias / scale follow the stacked-matrix row
+        const float bias = e.bias_m ? e.bias_m[mg] : 0.0f;
+        const float scl  = (e.scale_m ? e.scale_m[mg] : 1.0f) * e.alpha;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const int n = n0 + col + j;
-                if (mval && n < p.N) f[j] += e.res[roff + (int64_t) n * e.ldr + m];
-            }
-        }
-        if (!e.out_mmajor) {
-            if (e.out_f16 && e.hm_rows > 0) {                     // head-major: 64 consecutive features of a key are one 128-byte row
-                __half * o = reinterpret_cast<__half *>(e.out) + ooff + (int64_t) (m >> 6) * e.hm_rows * 64 + (m & 63);
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + col + j;
-                    if (mval && n < p.N) o[(int64_t) (n + e.n_row_off) * 64] = __float2half_rn(f[j]);
-                }
-            } else if (e.out_f16) {
-                __half * o = reinterpret_cast<__half *>(e.out) + ooff;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + col + j;
-                    if (mval && n < p.N) o[(int64_t) (n + e.n_row_off) * e.ldo + m] = __float2half_rn(f[j]);
-                }
-            } else {
-                float * o = reinterpret_cast<float *>(e.out) + ooff;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + col + j;
-                    if (mval && n < p.N) o[(int64_t) (n + e.n_row_off) * e.ldo + m] = f[j];
-                }
-            }
-        } else if (mval) {
-            const int nb = n0 + col;
-            const bool full = (nb + 32 <= p.N);
-            if (e.out_f16) {
-                __half * o = reinterpret_cast<__half *>(e.out) + ooff + (int64_t) m * e.ldo + nb;
-                if (full && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        __half2 h0 = __floats2half2_rn(f[j], f[j+1]),   h1 = __floats2half2_rn(f[j+2], f[j+3]);
-                        __half2 h2 = __floats2half2_rn(f[j+4], f[j+5]), h3 = __floats2half2_rn(f[j+6], f[j+7]);
-                        uint4 u = make_uint4(*reinterpret_cast<uint32_t *>(&h0), *reinterpret_cast<uint32_t *>(&h1),
-                                             *reinterpret_cast<uint32_t *>(&h2), *reinterpret_cast<uint32_t *>(&h3));
-                        *reinterpret_cast<uint4 *>(o + j) = u;
-                    }
-                } else {
-                    for (int j = 0; j < 32; ++j) if (nb + j < p.N) o[j] = __float2half_rn(f[j]);
-                }
-            } else {
-                float * o = reinterpret_cast<float *>(e.out) + ooff + (int64_t) m * e.ldo + nb;
-                if (full && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4 *>(o + j) = make_float4(f[j], f[j+1], f[j+2], f[j+3]);
-                } else {
-                    for (int j = 0; j < 32; ++j) if (nb + j < p.N) o[j] = f[j];
-                }
+            for (int c = 0; c < 2; ++c) {
+                const int n = n0 + 8 * j + 2 * (t & 3) + c;
+                if (n < p.N) epilogue_elem(e, ooff, roff, m, n, acc[4 * j + 2 * h + c], bias, scl);
             }
         }
     }
@@ -228,265 +139,124 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
     uint64_t * bars      = reinterpret_cast<uint64_t *>(sB + STAGES * Cfg::B_TILE_BYTES);
     uint64_t * full_bar  = bars;
     uint64_t * empty_bar = bars + STAGES;
-    uint64_t * accum_bar = bars + 2*STAGES;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 2*STAGES + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * 128;
-    const int n0 = blockIdx.y * BN;
-    const int b0 = blockIdx.z % p.nb0;
-    const int b1 = blockIdx.z / p.nb0;
-    const int nkb = p.taps * p.nkb_per_tap;
-    const int mg0 = m0 + b0 * p.a_rows_per_b0;     // first global A row of this tile (stacked weight matrices)
+    const int wg   = threadIdx.x >> 7;
+    const int nkb  = p.taps * p.nkb_per_tap;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmB);
         if (!QUANT) tma_prefetch_desc(&tmA);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full_bar[s], QUANT ? 1 + 8 : 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&full_bar[s], QUANT ? 1 + 4 : 1);      // TMA thread (+ the 4 decoder warps)
+            mbar_init(&empty_bar[s], 8);                     // the 8 consumer warps
         }
-        mbar_init(accum_bar, 1);
         mbar_fence_init();
     }
-    if (warp == 2) tmem_alloc<BN>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
-            int s = 0; uint32_t ph = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int tap = kb / p.nkb_per_tap;
-                const int k0  = (kb - tap * p.nkb_per_tap) * 64;
-                mbar_wait(&empty_bar[s], ph ^ 1);
-                const uint32_t tx = Cfg::B_TILE_BYTES + (QUANT ? 0 : A_TILE_BYTES);
-                mbar_arrive_expect_tx(&full_bar[s], tx);
-                const int sel[4] = { 0, b0, b1 + p.b1_in_off, tap };
-                tma_load_4d(sB + s * Cfg::B_TILE_BYTES, &tmB, &full_bar[s], k0, n0, sel[p.b_zsel0], sel[p.b_zsel1]);
-                if (!QUANT)
-                    tma_load_4d(sA + s * A_TILE_BYTES, &tmA, &full_bar[s], k0, mg0, sel[p.a_zsel0], sel[p.a_zsel1]);
-                if (++s == STAGES) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (single thread)
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_f16(128, BN);
-            int s = 0; uint32_t ph = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint64_t adesc = umma_desc_sw128(smem_u32(sA + s * A_TILE_BYTES));
-                const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + s * Cfg::B_TILE_BYTES));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    // +32 bytes per K=16 step inside the swizzle atom: +2 in the (addr >> 4) field
-                    umma_f16_ss(tmem_base, adesc + 2*k, bdesc + 2*k, idesc, (kb | k) ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[s]);
-                if (++s == STAGES) { s = 0; ph ^= 1; }
-            }
-            umma_commit(accum_bar);
-        }
-    } else {
-        // ------------------------------------------------------------------ warps 2..9
-        const int pt = threadIdx.x - 64;           // 0..255
-        if (QUANT) {
-            const int row  = pt >> 1;
-            const int half = pt & 1;
-            const int m    = mg0 + row;              // global row in the (stacked) weight matrix
-            const bool mval = (m0 + row) < p.M;
-            uint8_t * dst_row = sA + row * 128;
-            const int sw = row & 7;
-            int s = 0; uint32_t ph = 0;
-            if (WT == WT_Q4_K || WT == WT_Q5_K) {
-                constexpr int BLK = (WT == WT_Q4_K) ? 144 : 176;
-                const uint8_t * rowp = reinterpret_cast<const uint8_t *>(p.a_base) + (int64_t) m * (p.K >> 8) * BLK;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const int k = kb * 64 + half * 32;
-                    uint4 o[4];
-                    if (mval && k < p.K) {
-                        dequant_kq_sub<WT == WT_Q5_K>(rowp + (int64_t) (k >> 8) * BLK, (k & 255) >> 5, o);
-                    } else {
-                        o[0] = o[1] = o[2] = o[3] = make_uint4(0, 0, 0, 0);
-                    }
-                    mbar_wait(&empty_bar[s], ph ^ 1);
-                    uint8_t * d = dst_row + s * A_TILE_BYTES;
-#pragma unroll
-                    for (int c = 0; c < 4; ++c)
-                        *reinterpret_cast<uint4 *>(d + (((half * 4 + c) ^ sw) << 4)) = o[c];
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&full_bar[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
-                }
-            } else {
-                RawBlk r0, r1, r2;
-                raw_load<WT>(p, m, half * 32,      r0, mval && (half * 32      < p.K) && 0 < nkb);
-                raw_load<WT>(p, m, 64 + half * 32, r1, mval && (64 + half * 32 < p.K) && 1 < nkb);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const int k2 = (kb + 2) * 64 + half * 32;
-                    raw_load<WT>(p, m, k2, r2, mval && (kb + 2 < nkb) && (k2 < p.K));
-                    uint4 o[4];
-                    if (WT == WT_Q4_0)      dequant_q4_0(r0.q0, r0.d, o);
-                    else if (WT == WT_Q5_0) dequant_q5_0(r0.q0, r0.qh, r0.d, o);
-                    else                    dequant_q8_0(r0.q0, r0.q1, r0.d, o);
-                    mbar_wait(&empty_bar[s], ph ^ 1);
-                    uint8_t * d = dst_row + s * A_TILE_BYTES;
-#pragma unroll
-                    for (int c = 0; c < 4; ++c)
-                        *reinterpret_cast<uint4 *>(d + (((half * 4 + c) ^ sw) << 4)) = o[c];
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&full_bar[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
-                    r0 = r1; r1 = r2;
-                }
-            }
-        }
-
-        // ------------------------------------------------------------------ epilogue
-        mbar_wait(accum_bar, 0);
-        tc_fence_after();
-        gemm_epilogue_tile<BN>(p, tmem_base, m0, n0, b0, b1, warp, lane);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc<BN>(tmem_base);
-}
-
-// =============================================================================================== persistent f16 x f16 GEMM
-// Second generation of the encode-path GEMM.  Both operands are f16 tiles fetched by TMA (quantised weights are expanded ONCE per
-// launch into an f16 scratch by k_dequant_f16 -- a 128-row weight tile used to be re-decoded by every one of the up to 375 CTAs that
-// shared it), the kernel is PERSISTENT (one CTA per SM walks the tile list, weight-tile index fastest so that concurrently running CTAs
-// share activation tiles in L2) and the accumulator is DOUBLE-BUFFERED in tensor memory (2 x BN columns): the epilogue of tile i
-// (TMEM -> registers -> bias / GELU / residual -> global) overlaps the main loop of tile i+1.
-//   warp 0      : TMA producer   -- A and B tiles into a STAGES-deep smem ring (full / empty mbarriers)
-//   warp 1      : MMA issuer     -- one thread, 4 x tcgen05.mma (K = 16) per 64-wide k-block; commits the stage's "empty" barrier and,
-//                                   after the last k-block of a tile, the accumulator's "full" barrier
-//   warps 2..9  : epilogue       -- wait "full", drain the accumulator (gemm_epilogue_tile), arrive on its "empty" barrier
-// CL = 2: CTA PAIRS (thread-block cluster of 2 along the weight-row direction) share the activation tile: each CTA fetches HALF of it and
-// multicasts it into both CTAs' shared memory, so a CTA pulls 32 KB instead of 48 KB from L2 per k-block.  (Measured: the 1-CTA kernel
-// sits at ~0.8 of what L2 can feed -- 48 KB per 128 x 256 x 64 block at ~42 B/clk/SM is twice the 542 clocks the tensor pipe needs.)  A stage
-// is refilled only when BOTH CTAs have consumed it: the MMA thread's commit arrives on the "empty" barrier of both (count 2).
-template <int BN, int CL>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm2_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int n_mt, int n_nt, int n_tiles) {
-    using Cfg = GemmCfg<BN>;
-    constexpr int STAGES = Cfg::STAGES;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t * sA = smem;
-    uint8_t * sB = smem + STAGES * A_TILE_BYTES;
-    uint64_t * bars      = reinterpret_cast<uint64_t *>(sB + STAGES * Cfg::B_TILE_BYTES);
-    uint64_t * full_bar  = bars;
-    uint64_t * empty_bar = bars + STAGES;
-    uint64_t * tfull     = bars + 2*STAGES;          // [2] accumulator ready for the epilogue
-    uint64_t * tempty    = bars + 2*STAGES + 2;      // [2] accumulator drained
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 2*STAGES + 4);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int nkb = p.taps * p.nkb_per_tap;
-
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmB); tma_prefetch_desc(&tmA); }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 8); }
-        mbar_fence_init();
-    }
-    if (warp == 2) tmem_alloc<2 * BN>(tmem_slot);
-    tc_fence_before();
-    __syncthreads();
-    if (CL > 1) cluster_sync_all();                               // the peer's barriers exist before anything arrives on them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // tile list: with CL = 2 the CTAs of a pair take weight tiles 2q and 2q+1 of the same activation tile (n_mt is the number of PAIRS then)
-    const int crank = (CL > 1) ? (int) cluster_ctarank() : 0;
-    const int t_first = (CL > 1) ? (int) (blockIdx.x / CL) : (int) blockIdx.x, t_step = (int) gridDim.x / CL;
-
-    if (warp == 0) {
+    if (wg == 0) {
+        // ------------------------------------------------------------------ producer warpgroup
+        if (!QUANT && warp != 0) return;
+        const int row = threadIdx.x;                         // QUANT: weight row of the tile this thread decodes
         int s = 0; uint32_t ph = 0;
-        for (int t = t_first; t < n_tiles; t += t_step) {
-            const int mt = (t % n_mt) * CL + crank, r = t / n_mt, nt = r % n_nt, z = r / n_nt;
+        for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+            const int mt = t % p.n_mt, r = t / p.n_mt, nt = r % p.n_nt, z = r / p.n_nt;
             const int b0 = z % p.nb0, b1 = z / p.nb0;
-            const int mg0 = mt * 128 + b0 * p.a_rows_per_b0, n0 = nt * BN;
-            if (p.ep.res && lane > 0) {
+            const int m0 = mt * 128, mg0 = m0 + b0 * p.a_rows_per_b0, n0 = nt * BN;
+            if (warp == 0 && p.ep.res && lane > 0) {
                 // the residual tile (f32, 128 features of BN rows) goes to L2 while the tile's main loop runs: the epilogue then adds it at L2
-                // latency instead of stalling on HBM with only 32 KB in flight per SM
-                const int m0 = mt * 128, mw = min(128, p.M - m0);
+                // latency instead of stalling on HBM
+                const int mw = min(128, p.M - m0);
                 const float * rp = p.ep.res + (int64_t) b0 * p.ep.res_b0 + (int64_t) b1 * p.ep.res_b1 + m0;
                 if (mw > 0 && (mw & 3) == 0 && ((reinterpret_cast<uintptr_t>(rp) | ((uintptr_t) p.ep.ldr * 4)) & 15) == 0)
                     for (int rr = lane - 1; rr < BN && n0 + rr < p.N; rr += 31)
                         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(rp + (int64_t) (n0 + rr) * p.ep.ldr), "r"(mw * 4) : "memory");
             }
-            if (lane == 0) {
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const int tap = kb / p.nkb_per_tap;
-                    const int k0  = (kb - tap * p.nkb_per_tap) * 64;
+            const int m = mg0 + row;                         // QUANT: global row in the (stacked) weight matrix
+            const bool mval = (m0 + row) < p.M;
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int tap = kb / p.nkb_per_tap;
+                const int k0  = (kb - tap * p.nkb_per_tap) * 64;
+                if (threadIdx.x == 0) {
                     mbar_wait(&empty_bar[s], ph ^ 1);
-                    mbar_arrive_expect_tx(&full_bar[s], Cfg::B_TILE_BYTES + A_TILE_BYTES);
+                    mbar_arrive_expect_tx(&full_bar[s], Cfg::B_TILE_BYTES + (QUANT ? 0 : A_TILE_BYTES));
                     const int sel[4] = { 0, b0, b1 + p.b1_in_off, tap };
-                    if (CL > 1)                                    // my half of the activation tile, into both CTAs of the pair
-                        tma_load_4d_mc(sB + s * Cfg::B_TILE_BYTES + crank * (Cfg::B_TILE_BYTES / 2), &tmB, &full_bar[s], k0, n0 + crank * (BN / 2), sel[p.b_zsel0], sel[p.b_zsel1], (uint16_t) 3);
-                    else
-                        tma_load_4d(sB + s * Cfg::B_TILE_BYTES, &tmB, &full_bar[s], k0, n0, sel[p.b_zsel0], sel[p.b_zsel1]);
-                    tma_load_4d(sA + s * A_TILE_BYTES, &tmA, &full_bar[s], k0, mg0, sel[p.a_zsel0], sel[p.a_zsel1]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
+                    const int bh = BN / p.b_split;
+                    for (int i = 0; i < p.b_split; ++i)
+                        tma_load_4d(sB + s * Cfg::B_TILE_BYTES + i * bh * 128, &tmB, &full_bar[s], k0, n0 + i * bh, sel[p.b_zsel0], sel[p.b_zsel1]);
+                    if (!QUANT)
+                        tma_load_4d(sA + s * A_TILE_BYTES, &tmA, &full_bar[s], k0, mg0, sel[p.a_zsel0], sel[p.a_zsel1]);
                 }
-            }
-            __syncwarp();
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_f16(128, BN);
-            int s = 0; uint32_t ph = 0;
-            int i = 0;
-            for (int t = t_first; t < n_tiles; t += t_step, ++i) {
-                const int acc = i & 1;
-                mbar_wait(&tempty[acc], (uint32_t) ((i >> 1) & 1) ^ 1u);       // the epilogue has drained this accumulator (first use: free)
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + (uint32_t) (acc * BN);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    const uint64_t adesc = umma_desc_sw128(smem_u32(sA + s * A_TILE_BYTES));
-                    const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + s * Cfg::B_TILE_BYTES));
+                if (QUANT) {
+                    uint4 o[8];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ss(tacc, adesc + 2*k, bdesc + 2*k, idesc, (kb | k) ? 1u : 0u);
-                    if (CL > 1) umma_commit_mc(&empty_bar[s], (uint16_t) 3); else umma_commit(&empty_bar[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
+                    for (int hf = 0; hf < 2; ++hf) {
+                        const int k = kb * 64 + hf * 32;
+                        uint4 * oh = o + 4 * hf;
+                        if (!(mval && k < p.K)) {
+                            oh[0] = oh[1] = oh[2] = oh[3] = make_uint4(0, 0, 0, 0);
+                        } else if (WT == WT_Q4_K || WT == WT_Q5_K) {
+                            constexpr int BLK = (WT == WT_Q4_K) ? 144 : 176;
+                            const uint8_t * rowp = reinterpret_cast<const uint8_t *>(p.a_base) + (int64_t) m * (p.K >> 8) * BLK;
+                            uint4 q[4];
+                            dequant_kq_sub<WT == WT_Q5_K>(rowp + (int64_t) (k >> 8) * BLK, (k & 255) >> 5, q);
+                            oh[0] = q[0]; oh[1] = q[1]; oh[2] = q[2]; oh[3] = q[3];
+                        } else {
+                            RawBlk rb; uint4 q[4];
+                            raw_load<WT>(p, m, k, rb, true);
+                            if (WT == WT_Q4_0)      dequant_q4_0(rb.q0, rb.d, q);
+                            else if (WT == WT_Q5_0) dequant_q5_0(rb.q0, rb.qh, rb.d, q);
+                            else                    dequant_q8_0(rb.q0, rb.q1, rb.d, q);
+                            oh[0] = q[0]; oh[1] = q[1]; oh[2] = q[2]; oh[3] = q[3];
+                        }
+                    }
+                    mbar_wait(&empty_bar[s], ph ^ 1);
+                    uint8_t * d = sA + s * A_TILE_BYTES + row * 128;
+#pragma unroll
+                    for (int c = 0; c < 8; ++c)
+                        *reinterpret_cast<uint4 *>(d + ((c ^ (row & 7)) << 4)) = o[c];
+                    fence_proxy_async_smem();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&full_bar[s]);
                 }
-                umma_commit(&tfull[acc]);
+                if (++s == STAGES) { s = 0; ph ^= 1; }
             }
-        }
-    } else {
-        int i = 0;
-        for (int t = t_first; t < n_tiles; t += t_step, ++i) {
-            const int mt = (t % n_mt) * CL + crank, r = t / n_mt, nt = r % n_nt, z = r / n_nt;
-            const int b0 = z % p.nb0, b1 = z / p.nb0;
-            const int acc = i & 1;
-            mbar_wait(&tfull[acc], (uint32_t) ((i >> 1) & 1));
-            tc_fence_after();
-            gemm_epilogue_tile<BN>(p, tmem_base + (uint32_t) (acc * BN), mt * 128, nt * BN, b0, b1, warp, lane);
-            tc_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
         }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (CL > 1) cluster_sync_all();                               // nobody leaves while the peer may still multicast into it or arrive on its barriers
-    if (warp == 2) tmem_dealloc<2 * BN>(tmem_base);
+    // ------------------------------------------------------------------ consumer warpgroups
+    const int cw = wg - 1;                                   // rows 64*cw .. 64*cw + 63 of each 128-row weight tile
+    const int t128 = threadIdx.x & 127;
+    float acc[BN / 2];
+    int s = 0; uint32_t ph = 0;
+    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+        const int mt = t % p.n_mt, r = t / p.n_mt, nt = r % p.n_nt, z = r / p.n_nt;
+        const int b0 = z % p.nb0, b1 = z / p.nb0;
+        int s_prev = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(&full_bar[s], ph);
+            wgmma_fence();
+            const uint64_t adesc = wgmma_desc_sw128(smem_u32(sA + s * A_TILE_BYTES + cw * 64 * 128));
+            const uint64_t bdesc = wgmma_desc_sw128(smem_u32(sB + s * Cfg::B_TILE_BYTES));
+#pragma unroll
+            for (int k = 0; k < 4; ++k)                      // +32 bytes per K=16 step inside the swizzle atom: +2 in the (addr >> 4) field
+                wgmma_f16_ss<BN>(acc, adesc + 2*k, bdesc + 2*k, (kb | k) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();                                 // the previous k-block's MMAs are done: its stage can be refilled
+            wgmma_fence_regs(acc);
+            if (s_prev >= 0 && lane == 0) mbar_arrive(&empty_bar[s_prev]);
+            s_prev = s;
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (s_prev >= 0 && lane == 0) mbar_arrive(&empty_bar[s_prev]);
+        gemm_epilogue_regs<BN>(p, acc, mt * 128 + cw * 64, nt * BN, b0, b1, t128);
+    }
 }
 
 // expand a quantised matrix (planar 32-blocks or verbatim K-quant super-blocks) to f16 rows [rows][K]; one thread = one 32-value block.
@@ -549,49 +319,35 @@ bool make_tmap_f16(CUtensorMap * out, const void * base, uint64_t k, uint64_t ro
     return true;
 }
 
+static int gemm_n_sm() {
+    static int n = 0;
+    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceProp pr; if (cudaGetDeviceProperties(&pr, dev) == cudaSuccess) n = pr.multiProcessorCount; else n = 132; }
+    return n;
+}
+
+// persistent = false: one CTA per tile; true: one CTA per SM walking the tile list
 template <int BN, int WT>
-static cudaError_t launch_t(const GemmDesc & g, const GemmKParams & kp, cudaStream_t st) {
+static cudaError_t launch_t(const GemmDesc & g, GemmKParams kp, bool persistent, cudaStream_t st) {
     auto kern = gemm_kernel<BN, WT>;
     {
         const cudaError_t e = ensure_dyn_smem(reinterpret_cast<const void *>(kern), GemmCfg<BN>::SMEM);
         if (e != cudaSuccess) return e;
     }
-    dim3 grid((g.M + 127) / 128, (g.N + BN - 1) / BN, g.nb0 * g.nb1);
+    kp.n_mt = (g.M + 127) / 128; kp.n_nt = (g.N + BN - 1) / BN; kp.n_tiles = kp.n_mt * kp.n_nt * g.nb0 * g.nb1;
+    const int grid = persistent ? std::min(kp.n_tiles, gemm_n_sm()) : kp.n_tiles;
     kern<<<grid, GEMM_THREADS, GemmCfg<BN>::SMEM, st>>>(kp, g.tmA, g.tmB);
     count_launch();
     return cudaGetLastError();
 }
 
 template <int WT>
-static cudaError_t launch_bn(const GemmDesc & g, const GemmKParams & kp, cudaStream_t st) {
+static cudaError_t launch_bn(const GemmDesc & g, const GemmKParams & kp, bool persistent, cudaStream_t st) {
     switch (g.BN) {
-        case 64:  return launch_t<64,  WT>(g, kp, st);
-        case 128: return launch_t<128, WT>(g, kp, st);
-        case 256: return launch_t<256, WT>(g, kp, st);
+        case 64:  return launch_t<64,  WT>(g, kp, persistent, st);
+        case 128: return launch_t<128, WT>(g, kp, persistent, st);
+        case 256: return launch_t<256, WT>(g, kp, persistent, st);
     }
     return cudaErrorInvalidValue;
-}
-
-static int gemm_n_sm() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceProp pr; if (cudaGetDeviceProperties(&pr, dev) == cudaSuccess) n = pr.multiProcessorCount; else n = 148; }
-    return n;
-}
-
-template <int BN, int CL>
-static cudaError_t launch2_t(const GemmDesc & g, const GemmKParams & kp, cudaStream_t st) {
-    auto kern = gemm2_kernel<BN, CL>;
-    const size_t smem = GemmCfg<BN>::SMEM + 64;
-    { const cudaError_t e = ensure_dyn_smem(reinterpret_cast<const void *>(kern), smem); if (e != cudaSuccess) return e; }
-    const int n_mt = ((g.M + 127) / 128 + CL - 1) / CL, n_nt = (g.N + BN - 1) / BN, n_tiles = n_mt * n_nt * g.nb0 * g.nb1;   // CL = 2: pairs of weight tiles
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned) (CL * std::min(n_tiles, gemm_n_sm() / CL))); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = CL > 1 ? 1 : 0;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, kp, g.tmA, g.tmB, n_mt, n_nt, n_tiles);
-    count_launch();
-    return e;
 }
 
 cudaError_t dequant_to_f16(const QMat & W, int64_t rows, __half * out, cudaStream_t st) {
@@ -626,29 +382,19 @@ cudaError_t gemm_launch(const GemmDesc & g, cudaStream_t st) {
     kp.a_rows_per_b0 = g.a_rows_per_b0; kp.b1_in_off = g.b1_in_off;
     kp.a_base = g.A.base; kp.a_qs = g.A.qs; kp.a_qh = g.A.qh; kp.a_d = g.A.d;
     kp.ep = g.ep;
+    kp.b_split = g.half_box_b ? 2 : 1;
+    if (g.half_box_b && g.BN < 128) return cudaErrorInvalidValue;
     if (g.v2 && (g.A.type == WT_F16 || g.a16)) {                  // persistent kernel: both operands f16 through TMA
         if (g.A.type != WT_F16 && !g.a16_keep) { const cudaError_t e = dequant_launch(g, st); if (e != cudaSuccess) return e; }
-        if (g.cluster2) {                                          // tmB's box holds BN / 2 rows then
-            switch (g.BN) {
-                case 128: return launch2_t<128, 2>(g, kp, st);
-                case 256: return launch2_t<256, 2>(g, kp, st);
-            }
-            return cudaErrorInvalidValue;
-        }
-        switch (g.BN) {
-            case 64:  return launch2_t<64, 1>(g, kp, st);
-            case 128: return launch2_t<128, 1>(g, kp, st);
-            case 256: return launch2_t<256, 1>(g, kp, st);
-        }
-        return cudaErrorInvalidValue;
+        return launch_bn<WT_F16>(g, kp, true, st);
     }
     switch (g.A.type) {
-        case WT_F16:  return launch_bn<WT_F16>(g, kp, st);
-        case WT_Q4_0: return launch_bn<WT_Q4_0>(g, kp, st);
-        case WT_Q5_0: return launch_bn<WT_Q5_0>(g, kp, st);
-        case WT_Q8_0: return launch_bn<WT_Q8_0>(g, kp, st);
-        case WT_Q4_K: return launch_bn<WT_Q4_K>(g, kp, st);
-        case WT_Q5_K: return launch_bn<WT_Q5_K>(g, kp, st);
+        case WT_F16:  return launch_bn<WT_F16>(g, kp, false, st);
+        case WT_Q4_0: return launch_bn<WT_Q4_0>(g, kp, false, st);
+        case WT_Q5_0: return launch_bn<WT_Q5_0>(g, kp, false, st);
+        case WT_Q8_0: return launch_bn<WT_Q8_0>(g, kp, false, st);
+        case WT_Q4_K: return launch_bn<WT_Q4_K>(g, kp, false, st);
+        case WT_Q5_K: return launch_bn<WT_Q5_K>(g, kp, false, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -1,10 +1,10 @@
-// wb_gemm.cuh -- host-side description of one tcgen05 GEMM launch.
+// wb_gemm.cuh -- host-side description of one wgmma GEMM launch.
 //
 //   C[m][n] = sum_{tap} sum_{k} A[m][tap][k] * B[n][tap][k]            (both operands K-major, f16 in smem)
 //
-// "A" is the weight side: 128 rows per CTA land on the 128 TMEM lanes.  It is either an f16 matrix fetched by TMA
+// "A" is the weight side: 128 rows per CTA, 64 per MMA warpgroup.  It is either an f16 matrix fetched by TMA
 // or a quantised matrix (planar Q4_0/Q5_0/Q8_0, verbatim Q4_K/Q5_K) whose 32-value blocks are decoded to f16 by
-// the producer warps straight into the 128-byte-swizzled operand tile.
+// the producer warpgroup straight into the 128-byte-swizzled operand tile.
 // "B" is the activation side (tokens / time steps / queries): BN rows per CTA fetched by TMA.
 // This replaces ggml_mul_mat (ggml/src/ggml-cpu/ggml-cpu.c:1254-1452) + the separate add/scale/gelu/cpy nodes the
 // reference graphs attach to it (src/whisper.cpp:2119-2123, 2225-2239, 2309-2346, 2012-2020).
@@ -46,8 +46,8 @@ struct GemmDesc {
     QMat A;                           // weight side; type WT_F16 => tmA used
     CUtensorMap tmA;                  // valid when A.type == WT_F16, or when a16 is set (then it maps a16)
     __half * a16 = nullptr;           // quantised A: f16 scratch [rows][K] the persistent kernel's launch expands A into (shared by all launches of a stream)
-    int v2 = 0;                       // 1: persistent double-buffered kernel (gemm2_kernel)
-    int cluster2 = 0;                 // 1 (with v2): CTA pairs share the activation tile by TMA multicast; tmB must then be built with box_rows = BN / 2
+    int v2 = 0;                       // 1: persistent launch (one CTA per SM walks the tile list), A in f16 through TMA
+    int half_box_b = 0;               // 1: tmB was built with box_rows = BN / 2 (BN >= 128); the B tile is fetched as two halves
     int a16_keep = 0;                 // 1: a16 already holds this matrix (a launch sequence over the same weights expands them once)
     CUtensorMap tmB;
     GemmEpilogue ep;

@@ -1,4 +1,4 @@
-// wb_kernels.cu -- the bandwidth-bound kernels of the encode/decode path (everything that is not a tcgen05 GEMM).
+// wb_kernels.cu -- the bandwidth-bound kernels of the encode/decode path (everything that is not a wgmma GEMM).
 // Each kernel cites the reference lines whose arithmetic it reproduces.
 #include <cmath>
 #include <mutex>
@@ -27,7 +27,7 @@ __global__ void k_f16_to_f32(const __half * __restrict__ s, float * __restrict__
     const int64_t stride = (int64_t) gridDim.x * blockDim.x;
     for (; i < n; i += stride) d[i] = __half2float(s[i]);
 }
-static inline int grid_for(int64_t n, int tpb) { int64_t b = (n + tpb - 1) / tpb; return (int) (b < 148 * 16 ? (b > 0 ? b : 1) : 148 * 16); }
+static inline int grid_for(int64_t n, int tpb) { int64_t b = (n + tpb - 1) / tpb; return (int) (b < 132 * 16 ? (b > 0 ? b : 1) : 132 * 16); }
 void f32_to_f16(const float * src, __half * dst, int64_t n, cudaStream_t st) {
     if (n <= 0) return;
     k_f32_to_f16<<<grid_for(n, 256), 256, 0, st>>>(src, dst, n); count_launch();
@@ -648,7 +648,7 @@ static void gemv_launch(const GemvK & k, cudaStream_t st) {
     auto kern = k_gemv<WT, NT>;
     if (smem > 48 * 1024) ensure_dyn_smem(reinterpret_cast<const void *>(kern), smem);
     int grid = (N + 7) / 8;                  // one row per warp per pass
-    const int cap = 148 * 4;                 // keep the per-CTA prologue amortised over several rows
+    const int cap = 132 * 4;                 // keep the per-CTA prologue amortised over several rows
     if (grid > cap) grid = cap;
     kern<<<grid, 256, smem, st>>>(k); count_launch();
 }

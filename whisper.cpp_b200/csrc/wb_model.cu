@@ -385,8 +385,8 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
     }
     // Encoder-side matrices of a quantised model are kept a second time as f16 [N][K] (large-v3: 1.26 GB + 0.21 GB cross K/V projections
     // next to the 0.58 GB of blocks): the persistent tensor-core GEMM takes both operands through TMA, and a 30-s window multiplies every
-    // weight by 1500 activations -- expanding once at load instead of once per launch (or, first generation, once per CTA) is free on a
-    // 180 GB part.  WB200_ENC_F16=0 keeps only the blocks (the GEMM then expands each matrix into a scratch per launch).
+    // weight by 1500 activations -- expanding once at load instead of once per launch (or, first generation, once per CTA) costs 1.5 GB
+    // of the 80 GB.  WB200_ENC_F16=0 keeps only the blocks (the GEMM then expands each matrix into a scratch per launch).
     if (m.n_loaded > 0 && device >= 0 && m.wtype != WT_F16 && m.wtype != WT_F32 && !(getenv("WB200_ENC_F16") && atoi(getenv("WB200_ENC_F16")) == 0) &&
         getenv("WB200_GEMM_V1") == nullptr) {
         auto expand = [&](QMat & W) -> bool {

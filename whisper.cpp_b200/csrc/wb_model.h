@@ -1,4 +1,4 @@
-// wb_model.h -- the Whisper model as it lives on one B200: hyper-parameters, vocabulary (host) and weights (HBM).
+// wb_model.h -- the Whisper model as it lives on one GPU: hyper-parameters, vocabulary (host) and weights (HBM).
 //
 // File format: the legacy "ggml" container written by models/convert-pt-to-ggml.py:268-339 and read by
 // whisper_model_load (src/whisper.cpp:1485-1962): magic, 11 x i32 hparams, mel filters, vocabulary, then a stream

@@ -1,4 +1,4 @@
-// ggml_b200_backend.cpp -- ggml backend PLUGIN in front of the B200 engine (SURVEY.md section 8(b) "secondary seam", 8(f) rank 2).
+// ggml_b200_backend.cpp -- ggml backend PLUGIN in front of the engine (SURVEY.md section 8(b) "secondary seam", 8(f) rank 2).
 //
 // Built into libggml-b200.so and loaded by an UNMODIFIED reference program through GGML_BACKEND_PATH (ggml_backend_load_all,
 // reference ggml/src/ggml-backend-reg.cpp:562-591).  It implements the plugin interface of ggml/src/ggml-backend-impl.h:17-267:
@@ -332,7 +332,7 @@ ggml_backend_reg * the_reg();
 ggml_backend_device * the_dev();
 
 const char * dev_name(ggml_backend_dev_t) { return "B200"; }
-const char * dev_desc(ggml_backend_dev_t) { return "whisper.cpp_b200 engine (sm_100a) behind the ggml backend interface"; }
+const char * dev_desc(ggml_backend_dev_t) { return "whisper.cpp_b200 engine (sm_90a) behind the ggml backend interface"; }
 void dev_memory(ggml_backend_dev_t, size_t * free_b, size_t * total) { *free_b = (size_t) 160 << 30; *total = (size_t) 180 << 30; }
 enum ggml_backend_dev_type dev_type(ggml_backend_dev_t) { return GGML_BACKEND_DEVICE_TYPE_GPU; }
 void dev_props(ggml_backend_dev_t dev, ggml_backend_dev_props * p) {
