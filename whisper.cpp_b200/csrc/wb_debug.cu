@@ -201,4 +201,20 @@ int wb200_dbg_attn_cross(const float * q, const uint16_t * kc, const uint16_t * 
     return 0;
 }
 
+// W [N][K] in FILE layout -> tile-major records on the device (the decoder's layout) -> every element read back through the token-embedding
+// reader: out f32 [N][K]
+__attribute__((visibility("default")))
+int wb200_dbg_tm_dequant(int wtype, int N, int K, const void * w_file, float * out) {
+    if (wt_tm_rec_bytes(wtype) == 0 || K % wt_tm_rec_k(wtype) || K % 32) { set_error("wb200_dbg_tm_dequant: no tile-major layout for type %d, K=%d", wtype, K); return -5; }
+    DevBuf<uint8_t> wraw, tm; DevBuf<float> dout;
+    const size_t wbytes = (size_t) ((double) N * K * wt_bpw(wtype) + 0.5);
+    if (!wraw.alloc(wbytes) || !tm.alloc(wt_tm_bytes(wtype, N, K), true) || !dout.alloc((size_t) N * K)) return -1;
+    WB_CUDA_OKV(cudaMemcpy(wraw.p, w_file, wbytes, cudaMemcpyHostToDevice), -2);
+    QMat W; W.type = wtype; W.N = N; W.K = K; W.base = tm.p; W.layout = 1;
+    if (!repack_tile_major(wtype, wraw.p, W, 0, N, 0)) return -4;
+    dequant_rows_f32(W, dout.p, 0);
+    WB_CUDA_OKV(cudaMemcpy(out, dout.p, (size_t) N * K * 4, cudaMemcpyDeviceToHost), -2);
+    return 0;
+}
+
 } // extern "C"

@@ -6,7 +6,8 @@
 //               LN -> FC1 + GELU -> FC2 + residual
 //   then LN -> logits (token-embedding matrix).
 // The arithmetic per op is the one of the stand-alone kernels in wb_kernels.cu (Q8_0 activation blocks + integer block
-// dots like the reference CPU path, f16-rounded Q, f32 softmax); this file changes HOW the ops are scheduled:
+// dots like the reference CPU path -- Q8_K super-blocks for Q4_K / Q5_K weights --, f16-rounded Q, f32 softmax); this file changes HOW
+// the ops are scheduled:
 //   * grid = one CTA of 16 warps per SM, launched cooperatively; a phase boundary is a grid barrier instead of a kernel
 //     boundary (the decode step is a chain of ~400 dependent phases of a few microseconds each);
 //   * rows handed from one phase to the next are quantised once by their producer ("actq" rows in global memory): a
@@ -107,10 +108,42 @@ __device__ __noinline__ void mk_grid_sync(const MkArgs & a, unsigned long long t
 // Q8_0 rows follow quantize_row_q8_0 (d = amax/127 stored as f16, q = rint(x * 127/amax)); the two quotients are formed with a
 // reciprocal multiply / __fdividef: <= 2 ulp from the IEEE quotient, which only matters within 1e-6 of a rounding boundary.
 
-// one warp quantises the 32 values its lanes hold (one Q8_0 block of row t starting at element e0)
+// K-quant weights: rows are Q8_K (quantize_row_q8_K, ggml-quants.c:2768-2805, the arithmetic of k_act_quant<1>): int8 [64][K] followed
+// by one K/8-byte record per row (the size of the Q8_0 scales, so the staging is the same): f32 d[K/256] | int16 sum[K/32] of each
+// 32 quantised values (the dmin term).  A 256-value super-block needs its signed value of largest magnitude: producers that see
+// less than a super-block (attention heads, FC1 tiles) write f32 rows, and a quantise phase (mk_q8k_rows) follows them.
+constexpr bool mk_kq(int WT) { return WT == WT_Q4_K || WT == WT_Q5_K; }
+
+// the signed value of largest magnitude of two candidates; ties go to the larger value, so the choice does not depend on the order
+// (a tie between x and -x only flips the signs of q and d together)
+__device__ __forceinline__ void q8k_pick(float & amax, float & mx, float oa, float om) {
+    if (oa > amax || (oa == amax && om > mx)) { amax = oa; mx = om; }
+}
+__device__ __forceinline__ void q8k_warp_max(float & amax, float & mx) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) q8k_pick(amax, mx, __shfl_xor_sync(0xffffffffu, amax, o), __shfl_xor_sync(0xffffffffu, mx, o));
+}
+// q = min(127, nearest(iscale * x)) of four values, packed; `sum` gets their sum
+__device__ __forceinline__ uint32_t q8k_pack4(const float4 & y, float iscale, bool zero, int & sum) {
+    int q0 = 0, q1 = 0, q2 = 0, q3 = 0;
+    if (!zero) {
+        q0 = min(127, __float2int_rn(iscale * y.x)); q1 = min(127, __float2int_rn(iscale * y.y));
+        q2 = min(127, __float2int_rn(iscale * y.z)); q3 = min(127, __float2int_rn(iscale * y.w));
+    }
+    sum = (q0 + q1) + (q2 + q3);
+    return ((uint32_t) q0 & 0xffu) | (((uint32_t) q1 & 0xffu) << 8) | (((uint32_t) q2 & 0xffu) << 16) | ((uint32_t) q3 << 24);
+}
+__device__ __forceinline__ int sum8_lanes(int s) {              // over the 8 lanes of one 32-value sub-block (4 values per lane)
+    s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2); s += __shfl_xor_sync(0xffffffffu, s, 4);
+    return s;
+}
+__device__ __forceinline__ float * q8k_d(uint8_t * dst, int K, int row) { return reinterpret_cast<float *>(dst + (size_t) MK_MAXTOK * K + (size_t) row * (K >> 3)); }
+
+// one warp quantises the 32 values its lanes hold (one Q8_0 block of row t starting at element e0); K-quants: f32 store (see above)
 template <int WT>
 __device__ __forceinline__ void mk_store_q(uint8_t * dst, int K, int t, int e0, int lane, float v) {
     if (WT == WT_F16) { reinterpret_cast<__half *>(dst)[(size_t) t * K + e0 + lane] = __float2half_rn(v); return; }
+    if (mk_kq(WT)) { reinterpret_cast<float *>(dst)[(size_t) t * K + e0 + lane] = v; return; }
     const float amax = warp_max(fabsf(v));
     const float id = (amax != 0.0f) ? __fdividef(127.0f, amax) : 0.0f;
     reinterpret_cast<int8_t *>(dst)[(size_t) t * K + e0 + lane] = (int8_t) __float2int_rn(v * id);
@@ -138,7 +171,33 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const float * src, int K, 
         __syncthreads();
         q = (lane < MK_WARPS) ? SM_STAT[16 + lane] : 0.0f;
         const float rstd = 1.0f / sqrtf(warp_sum(q) / K + a.eps);
-        if (act) {
+        if (mk_kq(WT)) {                                         // Q8_K: a super-block is the 256 values of warps 2s, 2s + 1
+            float4 y = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if (act) {
+                const float4 w = __ldg(reinterpret_cast<const float4 *>(ln_w + e0)), b = __ldg(reinterpret_cast<const float4 *>(ln_b + e0));
+                y.x = __fadd_rn(__fmul_rn(__fmul_rn(v.x, rstd), w.x), b.x);
+                y.y = __fadd_rn(__fmul_rn(__fmul_rn(v.y, rstd), w.y), b.y);
+                y.z = __fadd_rn(__fmul_rn(__fmul_rn(v.z, rstd), w.z), b.z);
+                y.w = __fadd_rn(__fmul_rn(__fmul_rn(v.w, rstd), w.w), b.w);
+            }
+            float amax = fabsf(y.x), mx = y.x;
+            q8k_pick(amax, mx, fabsf(y.y), y.y); q8k_pick(amax, mx, fabsf(y.z), y.z); q8k_pick(amax, mx, fabsf(y.w), y.w);
+            q8k_warp_max(amax, mx);
+            if (lane == 0) { SM_PART[2 * warp] = amax; SM_PART[2 * warp + 1] = mx; }
+            __syncthreads();
+            if (act) {
+                const int w0 = warp & ~1;
+                amax = SM_PART[2 * w0]; mx = SM_PART[2 * w0 + 1];
+                q8k_pick(amax, mx, SM_PART[2 * w0 + 2], SM_PART[2 * w0 + 3]);
+                const float iscale = (amax != 0.0f) ? -127.0f / mx : 0.0f;
+                int s;
+                *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0) = q8k_pack4(y, iscale, amax == 0.0f, s);
+                s = sum8_lanes(s);
+                float * dd = q8k_d(dst, K, row);
+                if ((lane & 7) == 0) reinterpret_cast<short *>(dd + (K >> 8))[e0 >> 5] = (short) s;
+                if (lane == 0 && (warp & 1) == 0) dd[e0 >> 8] = (amax != 0.0f) ? 1.0f / iscale : 0.0f;
+            }
+        } else if (act) {
             const float4 w = __ldg(reinterpret_cast<const float4 *>(ln_w + e0)), b = __ldg(reinterpret_cast<const float4 *>(ln_b + e0));
             float4 y;
             y.x = __fadd_rn(__fmul_rn(__fmul_rn(v.x, rstd), w.x), b.x);
@@ -192,6 +251,28 @@ __device__ __noinline__ void mk_q8_rows(const MkArgs & a, const float * src, int
     }
 }
 
+// K-quants: f32 rows -> Q8_K rows, one warp per (row, super-block); followed by a grid barrier
+__device__ __noinline__ void mk_q8k_rows(const MkArgs & a, const float * src, int K, uint8_t * dst) {
+    const int lane = threadIdx.x & 31, nsb = K >> 8, n = a.n_tok * nsb;
+    for (int p = blockIdx.x * MK_WARPS + (threadIdx.x >> 5); p < n; p += gridDim.x * MK_WARPS) {
+        const int row = p / nsb, e0 = (p - row * nsb) * 256 + lane * 4;
+        const float4 y0 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0));
+        const float4 y1 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0 + 128));
+        float amax = fabsf(y0.x), mx = y0.x;
+        q8k_pick(amax, mx, fabsf(y0.y), y0.y); q8k_pick(amax, mx, fabsf(y0.z), y0.z); q8k_pick(amax, mx, fabsf(y0.w), y0.w);
+        q8k_pick(amax, mx, fabsf(y1.x), y1.x); q8k_pick(amax, mx, fabsf(y1.y), y1.y); q8k_pick(amax, mx, fabsf(y1.z), y1.z); q8k_pick(amax, mx, fabsf(y1.w), y1.w);
+        q8k_warp_max(amax, mx);
+        const float iscale = (amax != 0.0f) ? -127.0f / mx : 0.0f;
+        int s0, s1;
+        *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0)       = q8k_pack4(y0, iscale, amax == 0.0f, s0);
+        *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0 + 128) = q8k_pack4(y1, iscale, amax == 0.0f, s1);
+        s0 = sum8_lanes(s0); s1 = sum8_lanes(s1);
+        float * dd = q8k_d(dst, K, row);
+        if ((lane & 7) == 0) { short * ss = reinterpret_cast<short *>(dd + (K >> 8)); ss[e0 >> 5] = (short) s0; ss[(e0 >> 5) + 4] = (short) s1; }
+        if (lane == 0) dd[e0 >> 8] = (amax != 0.0f) ? 1.0f / iscale : 0.0f;
+    }
+}
+
 // TMA bulk copy global -> shared, completion on an mbarrier
 __device__ __forceinline__ void bulk_g2s(void * dst, const void * src, uint32_t bytes, uint64_t * bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -229,7 +310,8 @@ __device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_all;
 // 2.4 us for three slots): an iteration with four slots makes two calls of two slots, same partials, no spills.
 template <int WT, int NV, int TU, int KS, int UB>
 __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * wbase, int tile0, int tstep, int nrec, int nb, int SW, int nt, int NH, bool & staged, uint32_t stage_parity, int fb, int j0) {
-    constexpr int REC = (WT == WT_Q4_0) ? 288 : (WT == WT_Q5_0 ? 352 : (WT == WT_Q8_0 ? 544 : 512));
+    constexpr bool KQ = mk_kq(WT);
+    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 : 512));   // K-quants: bytes per 32 values
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RLD = 17;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3, ks = warp & (KS - 1);
@@ -239,13 +321,21 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 #pragma unroll
         for (int h = 0; h < 2; ++h) { acc[j][h][0] = acc[j][h][1] = acc[j][h][2] = acc[j][h][3] = 0.0f; }
     for (int kb = ks; kb < nrec; kb += KS * UB) {
-        uint4 wq[NV][UB]; uint2 wh[NV][UB]; uint32_t wd[NV][UB];
+        uint4 wq[NV][UB]; uint2 wh[NV][UB]; uint32_t wd[NV][UB]; uint2 wk[NV][UB];
 #pragma unroll
         for (int j = 0; j < NV; ++j) {
             {
                 const uint8_t * tb = wbase + (size_t) ((tile0 + ((j0 + j) / TU) * tstep) * TU + (j0 + j) % TU) * nrec * REC;
 #pragma unroll
                 for (int u = 0; u < UB; ++u) {
+                    if (KQ) {                                    // sub-block record of super-block sb (wb_quant.cuh) + this lane's 8 header bytes
+                        const int bb = min(kb + u * KS, nrec - 1);
+                        const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
+                        const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[j][u].x = q2.x; wq[j][u].y = q2.y;
+                        if (WT == WT_Q5_K) wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + 256) + g);
+                        wk[j][u] = __ldg(reinterpret_cast<const uint2 *>(sbp + 16 * (g + 8 * (c >> 1))) + (c & 1));
+                        continue;
+                    }
                     const uint8_t * rec = tb + (size_t) min(kb + u * KS, nrec - 1) * REC;
                     if (WT == WT_F16 || WT == WT_Q8_0) wq[j][u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
                     else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[j][u].x = q2.x; wq[j][u].y = q2.y; }
@@ -259,17 +349,44 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
         for (int u = 0; u < UB; ++u) {
             const int b = kb + u * KS;
             if (b < nrec) {
-                uint32_t bf[2][2]; float dx[2][2];
+                uint32_t bf[2][2]; float dx[2][2], sx[2][2];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const bool ok = h * 8 + g < nt;
                     bf[h][0] = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u;
                     bf[h][1] = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
                     dx[h][0] = dx[h][1] = 0.0f;
-                    if (WT != WT_F16) { dx[h][0] = SM_XD[min(h * 8 + 2 * c, nt - 1) * nb + b]; dx[h][1] = SM_XD[min(h * 8 + 2 * c + 1, nt - 1) * nb + b]; }
+                    if (KQ) {                                    // Q8_K: d of the super-block, sum of the sub-block (mk_store_q comment)
+                        const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
+                        dx[h][0] = SM_XD[r0 * nb + (b >> 3)]; dx[h][1] = SM_XD[r1 * nb + (b >> 3)];
+                        sx[h][0] = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
+                        sx[h][1] = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+                    } else if (WT != WT_F16) { dx[h][0] = SM_XD[min(h * 8 + 2 * c, nt - 1) * nb + b]; dx[h][1] = SM_XD[min(h * 8 + 2 * c + 1, nt - 1) * nb + b]; }
                 }
 #pragma unroll
                 for (int j = 0; j < NV; ++j) {
+                    if (KQ) {                                    // unsigned 4 / 5-bit weights; acc += d_x * (d sc_j * sumi - dmin m_j * sumx) as the chain
+                        uint32_t af[4];
+                        af[0] = wq[j][u].x & 0x0F0F0F0Fu; af[2] = (wq[j][u].x >> 4) & 0x0F0F0F0Fu;
+                        af[1] = wq[j][u].y & 0x0F0F0F0Fu; af[3] = (wq[j][u].y >> 4) & 0x0F0F0F0Fu;
+                        if (WT == WT_Q5_K) {
+                            af[0] |= spread4_to_bit4(wh[j][u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[j][u].x >> (16 + 4 * c));
+                            af[1] |= spread4_to_bit4(wh[j][u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[j][u].y >> (16 + 4 * c));
+                        }
+                        float dl0, ml0, dl1, ml1;
+                        kq_tm_scales(wk[j][u], b & 7, c, dl0, ml0, dl1, ml1);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            if (h < NH) {
+                                int dd[4]; mma_s8_16832(dd, af, bf[h][0], bf[h][1]);
+                                acc[j][h][0] = fmaf(dx[h][0], fmaf(dl0, (float) dd[0], -ml0 * sx[h][0]), acc[j][h][0]);
+                                acc[j][h][1] = fmaf(dx[h][1], fmaf(dl0, (float) dd[1], -ml0 * sx[h][1]), acc[j][h][1]);
+                                acc[j][h][2] = fmaf(dx[h][0], fmaf(dl1, (float) dd[2], -ml1 * sx[h][0]), acc[j][h][2]);
+                                acc[j][h][3] = fmaf(dx[h][1], fmaf(dl1, (float) dd[3], -ml1 * sx[h][1]), acc[j][h][3]);
+                            }
+                        }
+                        continue;
+                    }
                     {
                         uint32_t af[4];
                         float dw0 = 0.0f, dw1 = 0.0f;
@@ -379,7 +496,13 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const QMat & W, const uin
             switch (nv) {
                 case 1: if (!PAIR) { mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
                 case 2: mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break;
-                case 3: if (!PAIR) { mk_gemv_kloop<WT, 3, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
+                case 3:
+                    if (!PAIR && mk_kq(WT)) {                    // K-quant records carry a header share (and Q5_K fifth bits): two slots + one
+                        mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0);
+                        mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 2);
+                        break;
+                    }
+                    if (!PAIR) { mk_gemv_kloop<WT, 3, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
                 default:                                         // four slots: two passes of two (see mk_gemv_kloop)
                     mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0);
                     mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 2);
@@ -443,7 +566,8 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const QMat & W, const uin
 // is one accumulator over the blocks in ascending order: independent of the batch.
 template <int WT>
 __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const QMat & W, const uint8_t * x, float * out) {
-    constexpr int REC = (WT == WT_Q4_0) ? 288 : (WT == WT_Q5_0 ? 352 : (WT == WT_Q8_0 ? 544 : 512));
+    constexpr bool KQ = mk_kq(WT);
+    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 : 512));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RK = (WT == WT_F16) ? 16 : 32;
     constexpr int UB = 8;
@@ -479,9 +603,17 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const QMat & W, co
         for (int h = 0; h < 2; ++h) { acc[h][0] = acc[h][1] = acc[h][2] = acc[h][3] = 0.0f; }
         const uint8_t * tb = wbase + (size_t) tile * nrec * REC;
         for (int kb = 0; kb < nrec; kb += UB) {
-            uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB];
+            uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB]; uint2 wk[UB];
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
+                if (KQ) {
+                    const int bb = min(kb + u, nrec - 1);
+                    const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
+                    const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[u].x = q2.x; wq[u].y = q2.y;
+                    if (WT == WT_Q5_K) wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + 256) + g);
+                    wk[u] = __ldg(reinterpret_cast<const uint2 *>(sbp + 16 * (g + 8 * (c >> 1))) + (c & 1));
+                    continue;
+                }
                 const uint8_t * rec = tb + (size_t) min(kb + u, nrec - 1) * REC;
                 if (WT == WT_F16 || WT == WT_Q8_0) wq[u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
                 else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[u].x = q2.x; wq[u].y = q2.y; }
@@ -492,7 +624,33 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const QMat & W, co
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
                 const int b = kb + u;
-                if (b < nrec) {
+                if (KQ && b < nrec) {
+                    uint32_t af[4];
+                    af[0] = wq[u].x & 0x0F0F0F0Fu; af[2] = (wq[u].x >> 4) & 0x0F0F0F0Fu;
+                    af[1] = wq[u].y & 0x0F0F0F0Fu; af[3] = (wq[u].y >> 4) & 0x0F0F0F0Fu;
+                    if (WT == WT_Q5_K) {
+                        af[0] |= spread4_to_bit4(wh[u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[u].x >> (16 + 4 * c));
+                        af[1] |= spread4_to_bit4(wh[u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[u].y >> (16 + 4 * c));
+                    }
+                    float dl0, ml0, dl1, ml1;
+                    kq_tm_scales(wk[u], b & 7, c, dl0, ml0, dl1, ml1);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (h < NH) {
+                            const bool ok = h * 8 + g < nt;
+                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
+                            const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
+                            const float dx0 = SM_XD[r0 * nb + (b >> 3)], dx1 = SM_XD[r1 * nb + (b >> 3)];
+                            const float sx0 = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
+                            const float sx1 = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+                            int dd[4]; mma_s8_16832(dd, af, b0, b1);
+                            acc[h][0] = fmaf(dx0, fmaf(dl0, (float) dd[0], -ml0 * sx0), acc[h][0]);
+                            acc[h][1] = fmaf(dx1, fmaf(dl0, (float) dd[1], -ml0 * sx1), acc[h][1]);
+                            acc[h][2] = fmaf(dx0, fmaf(dl1, (float) dd[2], -ml1 * sx0), acc[h][2]);
+                            acc[h][3] = fmaf(dx1, fmaf(dl1, (float) dd[3], -ml1 * sx1), acc[h][3]);
+                        }
+                    }
+                } else if (!KQ && b < nrec) {
                     uint32_t af[4];
                     float dw0 = 0.0f, dw1 = 0.0f;
                     if (WT == WT_F16 || WT == WT_Q8_0) { af[0] = wq[u].x; af[1] = wq[u].y; af[2] = wq[u].z; af[3] = wq[u].w; }
@@ -696,7 +854,7 @@ __device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkLayer & L) {
         {
             float M, Lsum;
             const float o = attn_merge(SM_PART + grp * WPI * MK_PART, WPI, hw * 32 + lane, M, Lsum);
-            mk_store_q<WT>(a.actq, d, t, h * 64 + hw * 32, lane, (Lsum > 0.0f) ? __fdividef(o, Lsum) : 0.0f);
+            mk_store_q<WT>(mk_kq(WT) ? reinterpret_cast<uint8_t *>(a.q2) : a.actq, d, t, h * 64 + hw * 32, lane, (Lsum > 0.0f) ? __fdividef(o, Lsum) : 0.0f);
         }
         bar_named(1 + grp, WPI * 32);
     }
@@ -798,7 +956,7 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) 
             const int dim = warp * 32 + lane;
             float M, Lsum;
             const float o = attn_merge(SM_PART + buf * MK_WARPS * MK_PART, MK_WARPS, dim, M, Lsum);
-            mk_store_q<WT>(a.actq, d, t, h * 64 + warp * 32, lane, __fdividef(o, Lsum));
+            mk_store_q<WT>(mk_kq(WT) ? reinterpret_cast<uint8_t *>(a.qkv) : a.actq, d, t, h * 64 + warp * 32, lane, __fdividef(o, Lsum));
         }
         buf ^= 1;
         lane_init(A);
@@ -809,6 +967,7 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) 
 }
 
 #define MK_SYNC() do { MK_STAMP(); target += gridDim.x; mk_grid_sync(a, target); MK_STAMP(); } while (0)
+#define MK_SYNC_Q() do { target += gridDim.x; mk_grid_sync(a, target); } while (0)      // without trace stamps (24 per layer for every format)
 
 template <int WT, bool TRACE>
 __global__ void __launch_bounds__(MK_THREADS, 1)
@@ -836,6 +995,7 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
         // 3: self-attention (2603-2625) -> quantised rows for the O projection
         if (pf_w) mk_prefetch_w(L.cq);
         mk_attn_self<WT>(a, L);
+        if (mk_kq(WT)) { MK_SYNC_Q(); mk_q8k_rows(a, a.q2, d, a.actq); }     // K-quants: f32 rows -> Q8_K (timed with the attention)
         MK_SYNC();
         // 4: O + residual (2647-2659)
         if (pf_w) mk_prefetch_w(L.co);
@@ -853,6 +1013,7 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
         // 7: cross-attention (2688-2705)
         if (pf_w) mk_prefetch_w(L.fc2);
         mk_attn_cross<WT>(a, L);
+        if (mk_kq(WT)) { MK_SYNC_Q(); mk_q8k_rows(a, a.qkv, d, a.actq); }
         MK_SYNC();
         // 8: cross O + residual (2754-2766)
         e = MkEpi(); e.bias = L.co_bias; e.res = a.x; e.out = a.x;
@@ -863,9 +1024,16 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
         if (pf_w) { if (l + 1 < a.n_layer) mk_prefetch_w(a.layers[l + 1].qkv); else if (a.want_logits) mk_prefetch_w(a.te); }
         MK_SYNC();
         // 10: FC1 + GELU (2770-2794), then the rows are quantised for FC2
-        e = MkEpi(); e.bias = L.fc1_bias; e.act = 1; e.qout = a.hq;
-        mk_gemv<WT, true>(a, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
-        MK_STAMP(); MK_STAMP();                                  // (trace slot of the former FC1 -> Q8_0 phase)
+        if (mk_kq(WT)) {                                         // K-quants: f32 GELU rows, then a Q8_K phase (trace slot "10b h->q8")
+            e = MkEpi(); e.bias = L.fc1_bias; e.act = 1; e.out = a.h;
+            mk_gemv<WT, false>(a, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
+            MK_STAMP(); MK_SYNC_Q(); MK_STAMP();
+            mk_q8k_rows(a, a.h, 4 * d, a.hq);
+        } else {
+            e = MkEpi(); e.bias = L.fc1_bias; e.act = 1; e.qout = a.hq;
+            mk_gemv<WT, true>(a, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
+            MK_STAMP(); MK_STAMP();                              // (trace slot of the former FC1 -> Q8_0 phase)
+        }
         MK_SYNC();
         // 11: FC2 + residual (2797-2806)
         e = MkEpi(); e.bias = L.fc2_bias; e.res = a.x; e.out = a.x;
@@ -884,8 +1052,8 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
 bool mk_cross_head_major() {
     return true;
 }
-int mk_barriers(int n_layer, bool want_logits) { return 11 * n_layer + (want_logits ? 1 : 0); }
-bool mk_supported(int wtype) { return wtype == WT_F16 || wt_is_block32(wtype); }
+int mk_barriers(int wtype, int n_layer, bool want_logits) { return (wt_is_kquant(wtype) ? 14 : 11) * n_layer + (want_logits ? 1 : 0); }
+bool mk_supported(int wtype) { return wtype == WT_F16 || wt_is_block32(wtype) || wt_is_kquant(wtype); }
 size_t mk_smem_bytes(int, int) { return MK_SMEM; }
 int mk_max_rows() { return MK_MAXTOK; }
 
@@ -915,6 +1083,8 @@ bool mk_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st) {
         case WT_Q4_0: return WB_MK(WT_Q4_0);
         case WT_Q5_0: return WB_MK(WT_Q5_0);
         case WT_Q8_0: return WB_MK(WT_Q8_0);
+        case WT_Q4_K: return WB_MK(WT_Q4_K);
+        case WT_Q5_K: return WB_MK(WT_Q5_K);
         default: set_error("decode megakernel: unsupported weight type %d", wtype); return false;
     }
 #undef WB_MK

@@ -40,7 +40,7 @@ struct MkArgs {
 };
 
 // number of grid barriers one launch passes (host keeps bar_base in step)
-int  mk_barriers(int n_layer, bool want_logits);
+int  mk_barriers(int wtype, int n_layer, bool want_logits);
 bool mk_supported(int wtype);
 size_t mk_smem_bytes(int wtype, int d);
 bool mk_cross_head_major();        // cross K/V of a window is expected head-major ([layer][head][key][64])

@@ -520,7 +520,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
             mk_bar_total += 4096;
         } else {
             if (!mk_launch(a, m->wtype == WT_F32 ? WT_F16 : m->wtype, n_sm, st)) return false;
-            mk_bar_total += (unsigned long long) n_sm * mk_barriers(Lt, any_logits);
+            mk_bar_total += (unsigned long long) n_sm * mk_barriers(m->wtype == WT_F32 ? WT_F16 : m->wtype, Lt, any_logits);
         }
     } else
     for (int l = 0; l < Lt; ++l) {

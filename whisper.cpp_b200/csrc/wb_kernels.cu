@@ -123,9 +123,67 @@ __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restri
         }
     }
 }
+// K-quant tile-major records (wb_quant.cuh): one thread per (tile, 32-value sub-block, lane); the lanes of sub-block 0 also copy
+// the header (8 bytes each)
+template <int WT>
+__global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int rows, int K, int64_t n_threads) {
+    constexpr int BLK = (WT == WT_Q4_K) ? 144 : 176, QOFF = (WT == WT_Q4_K) ? 16 : 48;
+    const int REC = wt_tm_rec_bytes(WT), SUB = wt_tm_sub_bytes(WT), nsub = K / 32, nsb = K / 256;
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_threads) return;
+    const int lane = (int) (i & 31), g = lane >> 2, c = lane & 3;
+    const int64_t rb = i >> 5;
+    const int b = (int) (rb % nsub), sb = b >> 3, j = b & 7;
+    const int64_t tile = rb / nsub;
+    uint8_t * sbp = dst + (tile * nsb + sb) * REC;
+    uint8_t * rec = sbp + 256 + j * SUB;
+    const int64_t r0 = tile * 16 + g, r1 = r0 + 8;
+    auto blk = [&](int64_t r) { return src + (r * nsb + sb) * BLK; };
+    // bytes 4c .. 4c+3 of the row's 32 values in the Q4_0 order: byte i = q[i] | q[i + 16] << 4
+    auto word = [&](int64_t r) -> uint32_t {
+        if (r >= rows) return 0u;
+        const uint8_t * q = blk(r) + QOFF + 32 * (j >> 1);
+        const int sh = 4 * (j & 1);
+        uint32_t w = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int e = 4 * c + k;
+            w |= ((uint32_t) (((q[e] >> sh) & 0xF) | (((q[e + 16] >> sh) & 0xF) << 4))) << (8 * k);
+        }
+        return w;
+    };
+    reinterpret_cast<uint2 *>(rec)[lane] = make_uint2(word(r0), word(r1));
+    if (WT == WT_Q5_K && c == 0) {                               // fifth bits: bit e of the word = bit j of qh[e]
+        auto hbits = [&](int64_t r) -> uint32_t {
+            if (r >= rows) return 0u;
+            const uint8_t * qh = blk(r) + 16;
+            uint32_t h = 0;
+            for (int e = 0; e < 32; ++e) h |= (uint32_t) ((qh[e] >> j) & 1) << e;
+            return h;
+        };
+        reinterpret_cast<uint2 *>(rec + 256)[g] = make_uint2(hbits(r0), hbits(r1));
+    }
+    if (j == 0) {                                                // header: 16 bytes (d, dmin, scales) of each of the 16 rows
+        const int64_t r = tile * 16 + (lane >> 1);
+        uint32_t w[2] = { 0u, 0u };
+        if (r < rows) memcpy(w, blk(r) + 8 * (lane & 1), 8);
+        reinterpret_cast<uint2 *>(sbp)[lane] = make_uint2(w[0], w[1]);
+    }
+}
+
 bool repack_tile_major(int wtype, const uint8_t * src, const QMat & dst, int row_off, int rows, cudaStream_t st) {
     if (dst.layout != 1 || (row_off & 15)) { set_error("repack_tile_major: bad destination"); return false; }
     const int K = dst.K, nrec = K / wt_tm_rec_k(wtype);
+    if (wt_is_kquant(wtype)) {
+        const int64_t n_threads = (int64_t) ((rows + 15) / 16) * (K / 32) * 32;
+        if (n_threads == 0) return true;
+        uint8_t * out = const_cast<uint8_t *>(reinterpret_cast<const uint8_t *>(dst.base)) + (size_t) (row_off / 16) * nrec * wt_tm_rec_bytes(wtype);
+        const unsigned blocks = (unsigned) ((n_threads + 255) / 256);
+        if (wtype == WT_Q4_K) k_repack_tm_kq<WT_Q4_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads);
+        else                  k_repack_tm_kq<WT_Q5_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads);
+        count_launch();
+        return cudaGetLastError() == cudaSuccess;
+    }
     const int64_t tiles = (rows + 15) / 16, n_threads = tiles * nrec * 32;
     if (n_threads == 0) return true;
     uint8_t * out = const_cast<uint8_t *>(reinterpret_cast<const uint8_t *>(dst.base)) + (size_t) (row_off / 16) * nrec * wt_tm_rec_bytes(wtype);
@@ -341,6 +399,17 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
     const int REC = wt_tm_rec_bytes(W.type), rk = wt_tm_rec_k(W.type), nrec = W.K / rk;
     const int rr = (int) (row & 15), g = rr & 7, up = rr >> 3, i = e % rk;
     const uint8_t * rec = reinterpret_cast<const uint8_t *>(W.base) + ((row >> 4) * nrec + e / rk) * REC;
+    if (wt_is_kquant(W.type)) {                                  // dequantize_row_q4_K / _q5_K: (d * sc) * q - dmin * m, each product rounded
+        const uint8_t * hdr = rec + 16 * rr;
+        const int j = i >> 5, l = i & 31, c = (l & 15) >> 2;
+        int sc, mn; kq_scale_min(j, hdr + 4, sc, mn);
+        const float d = __half2float(*reinterpret_cast<const __half *>(hdr)), dmin = __half2float(*reinterpret_cast<const __half *>(hdr + 2));
+        const uint8_t * sub = rec + 256 + j * wt_tm_sub_bytes(W.type);
+        const uint32_t w = reinterpret_cast<const uint32_t *>(sub)[(g * 4 + c) * 2 + up];
+        int q = (int) ((w >> (8 * (l & 3) + 4 * (l >> 4))) & 0xFu);
+        if (W.type == WT_Q5_K) q |= (int) ((reinterpret_cast<const uint32_t *>(sub + 256)[g * 2 + up] >> l) & 1u) << 4;
+        return __fsub_rn(__fmul_rn(__fmul_rn(d, (float) sc), (float) q), __fmul_rn(dmin, (float) mn));
+    }
     if (W.type == WT_F16) {
         const int c = (i & 7) >> 1, k = up + ((i >> 3) << 1);
         const uint32_t w = reinterpret_cast<const uint32_t *>(rec)[(g * 4 + c) * 4 + k];
@@ -397,6 +466,14 @@ __global__ void k_dec_embed(const QMat te, const float * __restrict__ pe, const 
 }
 void dec_embed(const QMat & te, const float * pe, const int * tokens, const int * pos, int n_tok, int d, float * x, cudaStream_t st) {
     k_dec_embed<<<n_tok, 256, 0, st>>>(te, pe, tokens, pos, d, x); count_launch();
+}
+__global__ void k_dequant_rows(const QMat W, float * __restrict__ out) {
+    const int64_t n = (int64_t) W.N * W.K;
+    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x)
+        out[i] = dequant_elem(W, i / W.K, (int) (i % W.K));
+}
+void dequant_rows_f32(const QMat & W, float * out, cudaStream_t st) {
+    k_dequant_rows<<<1024, 256, 0, st>>>(W, out); count_launch();
 }
 
 // =====================================================================================================================

@@ -14,8 +14,11 @@ void f16_to_f32(const __half * src, float * dst, int64_t n, cudaStream_t st);
 bool repack_block32_into(int wtype, const uint8_t * file_blocks_dev, const QMat & dst, int rows, int K, cudaStream_t st);
 // convenience for tests: carve the planar arrays out of one buffer
 bool repack_block32(int wtype, const uint8_t * file_blocks_dev, uint8_t * dst, int N, int K, QMat * out, cudaStream_t st);
-// file-layout rows (32-blocks, or f16 rows for WT_F16) -> tile-major records (wb_quant.cuh) of `dst` (layout 1) starting at row row_off (multiple of 16)
+// file-layout rows (32-blocks, K-quant super-blocks, or f16 rows for WT_F16) -> tile-major records (wb_quant.cuh) of `dst` (layout 1)
+// starting at row row_off (multiple of 16)
 bool repack_tile_major(int wtype, const uint8_t * file_rows_dev, const QMat & dst, int row_off, int rows, cudaStream_t st);
+// every element of W through the embedding reader (dequant_elem): f32 [N][K] (test hook)
+void dequant_rows_f32(const QMat & W, float * out, cudaStream_t st);
 
 // ---- log-mel (src/whisper.cpp:3005-3272) ---------------------------------------------------------------------------
 // pcm: n_samples f32 on device.  mel: [n_mel][n_len] f32 with n_len = (n_samples + 480000)/160.  gmax: 1 float scratch.

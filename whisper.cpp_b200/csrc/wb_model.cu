@@ -48,7 +48,7 @@ void * dalloc(Model & m, size_t bytes, bool zero = true) {
 // allocate an [N][K] matrix of type t in its HBM layout
 bool alloc_qmat(Model & m, int t, int N, int K, QMat & q, bool tile_major = false) {
     q.type = t; q.N = N; q.K = K;
-    if (tile_major && wt_tm_rec_bytes(t) > 0 && K % 32 == 0) {
+    if (tile_major && wt_tm_rec_bytes(t) > 0 && K % 32 == 0 && K % wt_tm_rec_k(t) == 0) {
         const size_t bytes = wt_tm_bytes(t, N, K);
         q.base = dalloc(m, bytes);
         if (!q.base) return false;
@@ -130,7 +130,7 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
         default: set_error("invalid model (ftype %d is not supported by this engine)", hp.ftype); return false;
     }
     if (wt_is_kquant(m.wtype) && getenv("WB200_KQUANT_AS_F16") && atoi(getenv("WB200_KQUANT_AS_F16")) != 0) {
-        // opt-in: Q4_K / Q5_K run on the kernel chain (8 rows per decode pass); expanded to F16 they run in the persistent kernel (64 rows)
+        // opt-in: Q4_K / Q5_K expanded to F16 (2 bytes per weight, F16 arithmetic); without it their blocks decode natively (Q8_K activations)
         host_dq = m.wtype == WT_Q4_K ? HT_Q4_K : HT_Q5_K;
     }
     if (host_dq >= 0) {
@@ -221,9 +221,10 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
     };
     if (!add_ln("encoder.ln_post", m.e_ln) || !add_ln("decoder.ln", m.d_ln)) return false;
     {   // the persistent decode kernel (wb_decode_mk.cu) reads the decoder matrices in the tile-major layout; WB200_MEGAKERNEL=0
-        // keeps them planar for the kernel-per-op chain (K-quants and odd shapes always use the chain)
+        // keeps them planar for the kernel-per-op chain (odd shapes always use the chain; K-quants need whole super-blocks: d % 256)
         const char * e = getenv("WB200_MEGAKERNEL");
-        m.dec_tm = !m.force_planar && (!e || atoi(e) != 0) && wt_tm_rec_bytes(wt) > 0 && d % 128 == 0 && hp.n_text_head * 64 == d && hp.n_text_state == d;
+        m.dec_tm = !m.force_planar && (!e || atoi(e) != 0) && wt_tm_rec_bytes(wt) > 0 && d % 128 == 0 && (!wt_is_kquant(wt) || d % 256 == 0) &&
+                   hp.n_text_head * 64 == d && hp.n_text_state == d;
     }
     if (!alloc_qmat(m, wt, V, d, m.d_te, m.dec_tm)) return false;
     add_mat("decoder.token_embedding.weight", &m.d_te, 0, V, d);

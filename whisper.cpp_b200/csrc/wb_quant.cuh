@@ -11,7 +11,7 @@
 //     qh : [N][K/32]       uint32, the fifth bits (Q5_0 only)
 //     d  : [N][K/32]       f16 block scale
 // Total bytes are identical to the file (18 / 22 / 34 per 32 weights).  K-quant super-blocks are 144 / 176
-// bytes = multiples of 16 and are kept verbatim.
+// bytes = multiples of 16 and are kept verbatim (encoder side; the decoder matrices use the tile-major records below).
 #pragma once
 #include <cstdint>
 #include <cuda_fp16.h>
@@ -41,8 +41,17 @@ struct QMat {            // one weight matrix resident in HBM
 //   Q8_0 (544 B): u32 qs[32 lanes][4] = { w c / row g, w c / row g+8, w 4+c / row g, w 4+c / row g+8 } | f16 d[8][2]
 //   F16  (512 B per 16 values): u32 a[32 lanes][4] = the m16n8k16 A fragment
 // so one warp fetches a record with three fully coalesced loads.  Same bytes per weight as the file; rows >= N are zero.
-__host__ __device__ inline int wt_tm_rec_bytes(int t) { return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : 0; }
-__host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : 32; }
+// K-quants: one record per (tile, 256-value super-block), the 16 rows' super-blocks regrouped:
+//   Q4_K (2304 B): u8 hdr[16 rows][16] (the file's d, dmin, scales[12] of each row)   | 8 x sub-block record (256 B):
+//                  u32 qs[32 lanes][2] in the Q4_0 order, unsigned nibbles (byte i of a row's 16 = q[i] | q[i+16] << 4)
+//   Q5_K (2816 B): hdr as Q4_K | 8 x sub-block record (320 B): qs as Q4_K | u32 qh[8][2] = { row g, row g+8 } (bit i = fifth bit of q[i])
+// = the file's 16 x 144 / 16 x 176 bytes.  The GEMV splits K per 32-value sub-block (record + 256 + j * 256 / 320); a lane reads 8 bytes
+// of the header: lane 4g + c gets bytes 8 (c & 1) .. +7 of row g + 8 (c >> 1), so a quad holds the 32 header bytes of its two rows.
+__host__ __device__ inline int wt_tm_rec_bytes(int t) {
+    return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 : 0;
+}
+__host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : (t == WT_Q4_K || t == WT_Q5_K) ? 256 : 32; }
+__host__ __device__ inline int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : 320; }      // K-quants: one 32-value sub-block record
 __host__ __device__ inline size_t wt_tm_bytes(int t, int N, int K) { return (size_t) ((N + 15) / 16) * (K / wt_tm_rec_k(t)) * wt_tm_rec_bytes(t); }
 
 __host__ __device__ inline int wt_qs_bytes(int t)    { return t == WT_Q8_0 ? 32 : 16; }
@@ -123,6 +132,30 @@ __device__ __forceinline__ void dequant_q8_0(const uint4 q0, const uint4 q1, con
 __device__ __forceinline__ void kq_scale_min(int j, const uint8_t * q, int & sc, int & m) {
     if (j < 4) { sc = q[j] & 63; m = q[j + 4] & 63; }
     else       { sc = (q[j + 4] & 0xF) | ((q[j - 4] >> 6) << 4); m = (q[j + 4] >> 4) | ((q[j] >> 6) << 4); }
+}
+
+// tile-major K-quant records: (d * sc_j, dmin * m_j) of the rows g and g + 8 of the tile for sub-block j, from the 8 header bytes this lane
+// holds (layout above: lane 4g + c has bytes 8 (c & 1) .. + 7 of row g + 8 (c >> 1)).  Quad shuffles: the whole warp calls it with one j.
+__device__ __forceinline__ void kq_tm_scales(uint2 hp, int j, int c, float & dl0, float & ml0, float & dl1, float & ml1) {
+    const int sh = 8 * (j & 3);
+    uint32_t part;                                               // this lane's share of (sc | m << 8) of its row (get_scale_min_k4)
+    if (c & 1) {                                                 // hp = scales[4..7], scales[8..11]
+        const uint32_t bz = (hp.x >> sh) & 0xffu, bw = (hp.y >> sh) & 0xffu;
+        const uint32_t m = (j < 4) ? (bz & 63u) : ((bw >> 4) | ((bz >> 6) << 4));
+        part = ((j < 4) ? 0u : (bw & 0xFu)) | (m << 8);
+    } else {                                                     // hp = d | dmin << 16, scales[0..3]
+        const uint32_t by = (hp.y >> sh) & 0xffu;
+        part = (j < 4) ? (by & 63u) : ((by >> 6) << 4);
+    }
+    const uint32_t s  = part | __shfl_xor_sync(0xffffffffu, part, 1);
+    const uint32_t dp = __shfl_xor_sync(0xffffffffu, hp.x, 1);
+    const uint32_t dm = (c & 1) ? dp : hp.x;
+    const uint32_t s2 = __shfl_xor_sync(0xffffffffu, s, 2), dm2 = __shfl_xor_sync(0xffffffffu, dm, 2);
+    const uint32_t s0 = (c & 2) ? s2 : s, d0 = (c & 2) ? dm2 : dm, s1 = (c & 2) ? s : s2, d1 = (c & 2) ? dm : dm2;
+    dl0 = __half2float(__ushort_as_half((unsigned short) (d0 & 0xffffu))) * (float) (s0 & 0xffu);
+    ml0 = __half2float(__ushort_as_half((unsigned short) (d0 >> 16)))     * (float) (s0 >> 8);
+    dl1 = __half2float(__ushort_as_half((unsigned short) (d1 & 0xffffu))) * (float) (s1 & 0xffu);
+    ml1 = __half2float(__ushort_as_half((unsigned short) (d1 >> 16)))     * (float) (s1 >> 8);
 }
 
 // decode sub-block j (32 values) of a Q4_K / Q5_K super-block into 32 halves.
