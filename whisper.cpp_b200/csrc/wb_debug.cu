@@ -13,7 +13,8 @@ extern "C" {
 // C[n][m] (f32, token-major) = sum_k W[m][k] * X[n][k] ; W given in FILE layout (f16 rows or ggml quant blocks),
 // X given as f32 and rounded to f16 on the way in (as the engine does).  flags bit0: apply gelu; bit1: m-major output;
 // bit2: the persistent kernel (quantised weights expanded to f16 once, both operands through TMA); bit3: the activation tile fetched
-// as two half-height TMA boxes, bit4 = f16 output, bit5 = in-place f32 residual (out holds x on entry).
+// as two half-height TMA boxes, bit4 = f16 output, bit5 = in-place f32 residual (out holds x on entry), bit6 (with bit4, M a multiple of
+// 64) = head-major f16 output [M / 64][N][64] (the cross K/V layout), handed back in the token-major [N][M] view.
 __attribute__((visibility("default")))
 int wb200_dbg_gemm(int wtype, int M, int N, int K, const void * w_file, const float * x, const float * bias,
                    float * out, int BN, int flags) {
@@ -58,6 +59,10 @@ int wb200_dbg_gemm(int wtype, int M, int N, int K, const void * w_file, const fl
     if (flags & 16) {                                            // f16 output (token-major), widened to f32 for the caller
         if (!dout16.alloc((size_t) M * N)) return -1;
         g.ep.out = dout16.p; g.ep.out_f16 = 1;
+        if (flags & 64) {
+            if (M % 64 || (flags & 2)) { set_error("wb200_dbg_gemm: head-major output needs M %% 64 == 0 and token-major flags"); return -5; }
+            g.ep.hm_rows = N;
+        }
     }
     if (flags & 32) {                                            // in-place f32 residual: `out` holds x on entry, x + W a on return
         WB_CUDA_OKV(cudaMemcpy(dout.p, out, (size_t) M * N * 4, cudaMemcpyHostToDevice), -2);
@@ -70,6 +75,9 @@ int wb200_dbg_gemm(int wtype, int M, int N, int K, const void * w_file, const fl
     if (flags & 16) {
         std::vector<__half> h((size_t) M * N);
         WB_CUDA_OKV(cudaMemcpy(h.data(), dout16.p, (size_t) M * N * 2, cudaMemcpyDeviceToHost), -2);
+        if (flags & 64) {
+            for (int m = 0; m < M; ++m) for (int n = 0; n < N; ++n) out[(size_t) n * M + m] = __half2float(h[((size_t) (m / 64) * N + n) * 64 + (m % 64)]);
+        } else
         for (size_t i = 0; i < h.size(); ++i) out[i] = __half2float(h[i]);
         return 0;
     }

@@ -6,7 +6,10 @@
 //                                  for quantised A (first-generation launch) all 128 threads decode one weight row each (2 x 32-value
 //                                  blocks per 64-wide k-block) into the 128B-swizzled K-major operand tile
 //   warpgroups 1-2 : consumers  -- each owns 64 of the 128 weight rows: 4 x wgmma m64nBNk16 per k-block with the f32 accumulator in
-//                                  registers, then the epilogue (bias / scale / GELU / residual -> global) straight from those registers
+//                                  registers, then the epilogue (bias / scale / GELU / residual), staged through shared memory in 8 KB
+//                                  chunks and written with 16-byte stores
+// setmaxnreg moves registers from the producer warpgroup (40, 96 when it decodes quantised rows) to the consumers (232 / 200): no spills.
+// The epilogue kind (EpiKind) is a template parameter chosen at the launch site.
 // The same kernel serves the first-generation launch (one tile per CTA, quantised weights decoded in the kernel) and the persistent one
 // (gridDim = number of SMs, each CTA walks the tile list, weight-tile index fastest so that concurrently running CTAs share activation
 // tiles in L2; quantised weights expanded to f16 beforehand by k_dequant_f16, both operands through TMA).  The producer runs ahead into the
@@ -15,6 +18,7 @@
 //   * K-major SW128 tile: row r at byte r*128, 16-byte chunk c stored at chunk (c ^ (r & 7)); 8-row groups 1024 B apart
 //   * wgmma accumulator: thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8*j + 2*(t%4) (+1)
 #include <algorithm>
+#include <type_traits>
 #include "wb_gemm.cuh"
 #include "wb_ptx.cuh"
 #include "wb_common.h"
@@ -23,11 +27,14 @@ namespace wb {
 
 static constexpr int GEMM_THREADS  = 384;
 static constexpr int A_TILE_BYTES  = 128 * 64 * 2;
+// epilogue staging, per consumer warpgroup: one 8 KB chunk of output lines (see gemm_epilogue_regs) plus 16 bytes of padding per line,
+// so that the fragment writes of a warp spread over the banks
+static constexpr int EPI_STAGE_BYTES = 64 * (128 + 16);
 
 template <int BN> struct GemmCfg {
     static constexpr int B_TILE_BYTES = BN * 64 * 2;
     static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-    static constexpr int SMEM   = STAGES * (A_TILE_BYTES + B_TILE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int SMEM   = STAGES * (A_TILE_BYTES + B_TILE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * EPI_STAGE_BYTES;
 };
 
 struct GemmKParams {
@@ -70,20 +77,51 @@ __device__ __forceinline__ void raw_load(const GemmKParams & p, int m, int k, Ra
     }
 }
 
-// one accumulator value (weight row m, activation row n) through the epilogue; bias and scl belong to row m
-__device__ __forceinline__ void epilogue_elem(const GemmEpilogue & e, int64_t ooff, int64_t roff, int m, int n, float v, float bias, float scl) {
-    if (e.res && !e.out_mmajor && !e.out_f16 && e.act == 0) {
-        // f32 residual stream (attention-O / FC2: x += W a)
-        float * o = reinterpret_cast<float *>(e.out) + ooff;
-        o[(int64_t) (n + e.n_row_off) * e.ldo + m] = fmaf(v, scl, bias * scl) + __ldcg(e.res + roff + (int64_t) n * e.ldr + m);
-        return;
-    }
-    if (e.act == 1 && e.out_f16 && !e.res && !e.out_mmajor && e.hm_rows == 0) {
-        // FC1: GELU with the reference's f16 table semantics, a dozen instructions per value: see gelu_ref_f16 for the formula and its accuracy
+// Epilogue kinds: chosen on the host from the GemmEpilogue (epi_kind), so that the kernel carries no per-element flag tests.
+enum EpiKind : int {
+    EPI_F16          = 0,   // (acc + bias) * scl -> f16 out[n][m]                          (QK, cross K/V token-major)
+    EPI_F16_GELU     = 1,   // GELU(acc * scl + bias * scl) -> f16 out[n][m]               (FC1, conv1)
+    EPI_F32_RES      = 2,   // acc * scl + bias * scl + res[n][m] -> f32 out[n][m]         (attention-O, FC2: in place on the residual stream)
+    EPI_F16_MMAJOR   = 3,   // (acc + bias) * scl -> f16 out[m][n]                          (V^T)
+    EPI_F16_HM       = 4,   // (acc + bias) * scl -> f16 out[m / 64][n][m % 64]             (cross K/V head-major)
+    EPI_GENERAL      = 5,   // every flag of GemmEpilogue tested per value                  (conv2, the unfused attention, the test hook)
+};
+
+static EpiKind epi_kind(const GemmEpilogue & e) {
+    const bool plain = !e.res && !e.out_mmajor && e.hm_rows == 0;
+    if (e.out_f16 && plain && e.act == 0) return EPI_F16;
+    if (e.out_f16 && plain && e.act == 1) return EPI_F16_GELU;
+    if (e.res && !e.out_mmajor && !e.out_f16 && e.act == 0) return EPI_F32_RES;
+    if (e.out_f16 && e.out_mmajor && !e.res && e.act == 0) return EPI_F16_MMAJOR;
+    if (e.out_f16 && e.hm_rows > 0 && !e.out_mmajor && !e.res && e.act == 0) return EPI_F16_HM;
+    return EPI_GENERAL;
+}
+
+// the value of one accumulator (weight row m, activation row n) after the epilogue arithmetic of kind EK; bias and scl belong to row m
+template <int EK>
+__device__ __forceinline__ float epilogue_value(const GemmEpilogue & e, int64_t roff, int m, int n, float v, float bias, float scl) {
+    if constexpr (EK == EPI_F32_RES) {
+        return fmaf(v, scl, bias * scl) + __ldcg(e.res + roff + (int64_t) n * e.ldr + m);
+    } else if constexpr (EK == EPI_F16_GELU) {
+        // GELU with the reference's f16 table semantics, a dozen instructions per value: see gelu_ref_f16 for the formula and its accuracy
         float x = __half2float(__float2half_rn(fmaf(v, scl, bias * scl)));
         x = fmaxf(x, -20.0f);                                           // gelu = 0 below -10 either way; keeps exp finite
         const float ex = __expf(x * fmaf(x * x, -0.07135481627f, -1.5957691216f));
-        reinterpret_cast<__half *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = __float2half_rn(__fdividef(x, 1.0f + ex));
+        return __fdividef(x, 1.0f + ex);
+    } else {
+        return (v + bias) * scl;
+    }
+}
+
+// one accumulator value through the general epilogue: every flag tested, the residual and GELU kinds recognised per value (the
+// first-generation launch with quantised weights uses this for all kinds)
+__device__ __forceinline__ void epilogue_elem_general(const GemmEpilogue & e, int64_t ooff, int64_t roff, int m, int n, float v, float bias, float scl) {
+    if (e.res && !e.out_mmajor && !e.out_f16 && e.act == 0) {
+        reinterpret_cast<float *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = epilogue_value<EPI_F32_RES>(e, roff, m, n, v, bias, scl);
+        return;
+    }
+    if (e.act == 1 && e.out_f16 && !e.res && !e.out_mmajor && e.hm_rows == 0) {
+        reinterpret_cast<__half *>(e.out)[ooff + (int64_t) (n + e.n_row_off) * e.ldo + m] = __float2half_rn(epilogue_value<EPI_F16_GELU>(e, roff, m, n, v, bias, scl));
         return;
     }
     float x = (v + bias) * scl;
@@ -101,36 +139,159 @@ __device__ __forceinline__ void epilogue_elem(const GemmEpilogue & e, int64_t oo
     }
 }
 
-// epilogue of the 64 x BN accumulator of one consumer warpgroup (rows m0 .. m0 + 63 of the weight side, columns n0 .. n0 + BN - 1)
-template <int BN>
-__device__ __forceinline__ void gemm_epilogue_regs(const GemmKParams & p, const float (&acc)[BN / 2], int m0, int n0, int b0, int b1, int t) {
+template <typename T> __device__ __forceinline__ void store_pair(T * o, float lo, float hi);
+template <> __device__ __forceinline__ void store_pair<__half>(__half * o, float lo, float hi) { *reinterpret_cast<__half2 *>(o) = __floats2half2_rn(lo, hi); }
+template <> __device__ __forceinline__ void store_pair<float>(float * o, float lo, float hi) { *reinterpret_cast<float2 *>(o) = make_float2(lo, hi); }
+template <typename T> __device__ __forceinline__ T from_f32(float x);
+template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
+template <> __device__ __forceinline__ float  from_f32<float>(float x)  { return x; }
+
+// epilogue of the 64 x BN accumulator of one consumer warpgroup (rows m0 .. m0 + 63 of the weight side, columns n0 .. n0 + BN - 1).
+// Bias and scale are loaded once per row.  The general kind stores each value from its fragment position; the others go through the
+// warpgroup's staging buffer `stage` (below).  Only the grouping of the stores differs between the two: every value is computed by the
+// formula of its kind.
+template <int BN, int EK>
+__device__ __forceinline__ void gemm_epilogue_regs(const GemmKParams & p, const float (&acc)[BN / 2], int m0, int n0, int b0, int b1, int t,
+                                                   uint8_t * stage) {
     const GemmEpilogue & e = p.ep;
     const int64_t ooff = (int64_t) b0 * e.out_b0 + (int64_t) b1 * e.out_b1;
     const int64_t roff = (int64_t) b0 * e.res_b0 + (int64_t) b1 * e.res_b1;
+    if constexpr (EK == EPI_GENERAL) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int m = m0 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;
-        if (m >= p.M) continue;
-        const int mg = m + b0 * p.a_rows_per_b0;                        // bias / scale follow the stacked-matrix row
-        const float bias = e.bias_m ? e.bias_m[mg] : 0.0f;
-        const float scl  = (e.scale_m ? e.scale_m[mg] : 1.0f) * e.alpha;
+        for (int h = 0; h < 2; ++h) {
+            const int m = m0 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;
+            if (m >= p.M) continue;
+            const int mg = m + b0 * p.a_rows_per_b0;                    // bias / scale follow the stacked-matrix row
+            const float bias = e.bias_m ? e.bias_m[mg] : 0.0f;
+            const float scl  = (e.scale_m ? e.scale_m[mg] : 1.0f) * e.alpha;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const int n = n0 + 8 * j + 2 * (t & 3) + c;
-                if (n < p.N) epilogue_elem(e, ooff, roff, m, n, acc[4 * j + 2 * h + c], bias, scl);
+                for (int c = 0; c < 2; ++c) {
+                    const int n = n0 + 8 * j + 2 * (t & 3) + c;
+                    if (n < p.N) epilogue_elem_general(e, ooff, roff, m, n, acc[4 * j + 2 * h + c], bias, scl);
+                }
+            }
+        }
+    } else {
+        // Through shared memory: the warpgroup's 64 x BN block goes out in chunks of 8 KB.  A chunk is a set of output lines that are
+        // contiguous in global memory: for the n-major kinds one line = one activation row n with the warpgroup's 64 weight rows
+        // (64 f16 = 128 B, or 64 f32 = 256 B; 64 or 32 lines per chunk), for the m-major kind one line = one weight row m with 64
+        // columns n (128 B; 64 lines).  The fragments are written into the chunk, then the warpgroup copies it out with 16-byte stores.
+        using OutT = typename std::conditional<EK == EPI_F32_RES, float, __half>::type;
+        constexpr bool MMAJ  = (EK == EPI_F16_MMAJOR);
+        constexpr int  VB    = (int) sizeof(OutT);                        // bytes per value
+        constexpr int  VEC   = 16 / VB;                                   // values per 16-byte vector
+        constexpr int  LB    = 64 * VB;                                   // line bytes
+        constexpr int  LS    = LB + 16;                                   // line stride in shared memory
+        constexpr int  CN    = MMAJ ? 64 : 8192 / LB;                     // columns n per chunk
+        constexpr int  LINES = MMAJ ? 64 : CN;
+        static_assert(LINES * LS <= EPI_STAGE_BYTES, "epilogue chunk does not fit its staging buffer");
+        constexpr int  NCH   = (BN > CN) ? BN / CN : 1;
+        constexpr int  CJ    = ((BN < CN) ? BN : CN) / 8;                 // accumulator column groups per chunk
+        OutT * out = reinterpret_cast<OutT *>(e.out) + ooff;
+        const int bar_id = threadIdx.x >> 7;                              // one named barrier per consumer warpgroup (ids 1, 2)
+        // 16-byte accesses need every line start on a 16-byte boundary
+        bool vec = ((reinterpret_cast<uintptr_t>(e.out) & 15) == 0) && (ooff % VEC) == 0 && (EK == EPI_F16_HM || (e.ldo % VEC) == 0);
+        if constexpr (EK == EPI_F32_RES)
+            vec = vec && ((reinterpret_cast<uintptr_t>(e.res) & 15) == 0) && (roff % VEC) == 0 && (e.ldr % VEC) == 0;
+        const int odd = (t >> 2) & 1;                                     // parity of this lane's rows (m0 is a multiple of 64)
+        float bias[2], scl[2];
+        bool mval[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = m0 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;
+            mval[h] = m < p.M;
+            const int mg = m + b0 * p.a_rows_per_b0;                      // bias / scale follow the stacked-matrix row
+            bias[h] = (mval[h] && e.bias_m) ? e.bias_m[mg] : 0.0f;
+            scl[h]  = ((mval[h] && e.scale_m) ? e.scale_m[mg] : 1.0f) * e.alpha;
+        }
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+            bar_named(bar_id, 128);                                       // the previous chunk has been copied out
+#pragma unroll
+            for (int jj = 0; jj < CJ; ++jj) {
+                const int j = c * CJ + jj;
+                const int n = n0 + 8 * j + 2 * (t & 3);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int ml = 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;   // row inside the warpgroup's 64
+                    const int m = m0 + ml;
+                    float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                    // the residual is added in the copy-out (same f32 addition, same operands)
+                    constexpr int VK = (EK == EPI_F32_RES) ? -1 : EK;
+                    if (mval[h] && n < p.N) {
+                        if constexpr (VK < 0) x0 = fmaf(x0, scl[h], bias[h] * scl[h]);
+                        else                  x0 = epilogue_value<EK>(e, roff, m, n, x0, bias[h], scl[h]);
+                    }
+                    if (mval[h] && n + 1 < p.N) {
+                        if constexpr (VK < 0) x1 = fmaf(x1, scl[h], bias[h] * scl[h]);
+                        else                  x1 = epilogue_value<EK>(e, roff, m, n + 1, x1, bias[h], scl[h]);
+                    }
+                    if constexpr (MMAJ) {
+                        store_pair<OutT>(reinterpret_cast<OutT *>(stage + ml * LS) + 8 * jj + 2 * (t & 3), x0, x1);
+                    } else {
+                        // lanes t and t ^ 4 hold rows ml, ml ^ 1 of columns n, n + 1: after one exchange the even row's lane holds column n
+                        // of both rows and the odd row's lane column n + 1, i.e. two adjacent values of one line
+                        const float recv = __shfl_xor_sync(0xffffffffu, odd ? x0 : x1, 4);
+                        const float lo = odd ? recv : x0, hi = odd ? x1 : recv;
+                        store_pair<OutT>(reinterpret_cast<OutT *>(stage + (8 * jj + 2 * (t & 3) + odd) * LS) + (ml - odd), lo, hi);
+                    }
+                }
+            }
+            bar_named(bar_id, 128);                                       // the chunk is complete
+            constexpr int VPL = LB / 16;                                  // vectors per line
+#pragma unroll
+            for (int v = t; v < LINES * VPL; v += 128) {
+                const int line = v / VPL, q = v % VPL;
+                const OutT * src = reinterpret_cast<const OutT *>(stage + line * LS + q * 16);
+                OutT * dst;
+                int lim;                                                  // valid values of this vector
+                int64_t rrow = 0;
+                if constexpr (MMAJ) {
+                    const int m = m0 + line, n = n0 + c * CN + q * VEC;
+                    if (m >= p.M) continue;
+                    dst = out + (int64_t) m * e.ldo + n;
+                    lim = p.N - n;
+                } else {
+                    const int n = n0 + c * CN + line, m = m0 + q * VEC;
+                    if (n >= p.N) continue;
+                    dst = (EK == EPI_F16_HM) ? out + (int64_t) (m >> 6) * e.hm_rows * 64 + (int64_t) (n + e.n_row_off) * 64 + (m & 63)
+                                             : out + (int64_t) (n + e.n_row_off) * e.ldo + m;
+                    lim = p.M - m;
+                    rrow = roff + (int64_t) n * e.ldr + m;
+                }
+                if (lim <= 0) continue;
+                if constexpr (EK == EPI_F32_RES) {
+                    float4 x = *reinterpret_cast<const float4 *>(src);
+                    if (vec && lim >= VEC) {
+                        const float4 r = __ldcg(reinterpret_cast<const float4 *>(e.res + rrow));
+                        x.x += r.x; x.y += r.y; x.z += r.z; x.w += r.w;
+                        *reinterpret_cast<float4 *>(dst) = x;
+                    } else {
+                        const float xs[4] = { x.x, x.y, x.z, x.w };
+                        for (int i = 0; i < VEC && i < lim; ++i) dst[i] = xs[i] + __ldcg(e.res + rrow + i);
+                    }
+                } else {
+                    if (vec && lim >= VEC) *reinterpret_cast<uint4 *>(dst) = *reinterpret_cast<const uint4 *>(src);
+                    else for (int i = 0; i < VEC && i < lim; ++i) dst[i] = src[i];
+                }
             }
         }
     }
 }
 
-template <int BN, int WT>
+template <int BN, int WT, int EK>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB) {
     using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr bool QUANT = (WT != WT_F16);
+    // register split: the producer warpgroup (one TMA thread, or 128 row decoders for quantised weights) gives registers to the two
+    // consumer warpgroups, which hold BN / 2 accumulators each.  128 * P + 256 * C = 64512 = 384 * 168, the budget at launch.
+    constexpr int REGS_PRODUCER = QUANT ? 96 : 40;
+    constexpr int REGS_CONSUMER = QUANT ? 200 : 232;
+    static_assert(128 * REGS_PRODUCER + 256 * REGS_CONSUMER <= 384 * 168, "register split over budget");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -158,6 +319,7 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
 
     if (wg == 0) {
         // ------------------------------------------------------------------ producer warpgroup
+        reg_dealloc<REGS_PRODUCER>();                        // all four warps, before any of them leaves
         if (!QUANT && warp != 0) return;
         const int row = threadIdx.x;                         // QUANT: weight row of the tile this thread decodes
         int s = 0; uint32_t ph = 0;
@@ -229,7 +391,9 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
     }
 
     // ------------------------------------------------------------------ consumer warpgroups
+    reg_alloc<REGS_CONSUMER>();
     const int cw = wg - 1;                                   // rows 64*cw .. 64*cw + 63 of each 128-row weight tile
+    uint8_t * epi_stage = reinterpret_cast<uint8_t *>(bars) + 256 + cw * EPI_STAGE_BYTES;
     const int t128 = threadIdx.x & 127;
     float acc[BN / 2];
     int s = 0; uint32_t ph = 0;
@@ -255,7 +419,7 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         if (s_prev >= 0 && lane == 0) mbar_arrive(&empty_bar[s_prev]);
-        gemm_epilogue_regs<BN>(p, acc, mt * 128 + cw * 64, nt * BN, b0, b1, t128);
+        gemm_epilogue_regs<BN, EK>(p, acc, mt * 128 + cw * 64, nt * BN, b0, b1, t128, epi_stage);
     }
 }
 
@@ -326,9 +490,9 @@ static int gemm_n_sm() {
 }
 
 // persistent = false: one CTA per tile; true: one CTA per SM walking the tile list
-template <int BN, int WT>
+template <int BN, int WT, int EK>
 static cudaError_t launch_t(const GemmDesc & g, GemmKParams kp, bool persistent, cudaStream_t st) {
-    auto kern = gemm_kernel<BN, WT>;
+    auto kern = gemm_kernel<BN, WT, EK>;
     {
         const cudaError_t e = ensure_dyn_smem(reinterpret_cast<const void *>(kern), GemmCfg<BN>::SMEM);
         if (e != cudaSuccess) return e;
@@ -340,14 +504,33 @@ static cudaError_t launch_t(const GemmDesc & g, GemmKParams kp, bool persistent,
     return cudaGetLastError();
 }
 
-template <int WT>
+template <int WT, int EK>
 static cudaError_t launch_bn(const GemmDesc & g, const GemmKParams & kp, bool persistent, cudaStream_t st) {
     switch (g.BN) {
-        case 64:  return launch_t<64,  WT>(g, kp, persistent, st);
-        case 128: return launch_t<128, WT>(g, kp, persistent, st);
-        case 256: return launch_t<256, WT>(g, kp, persistent, st);
+        case 64:  return launch_t<64,  WT, EK>(g, kp, persistent, st);
+        case 128: return launch_t<128, WT, EK>(g, kp, persistent, st);
+        case 256: return launch_t<256, WT, EK>(g, kp, persistent, st);
     }
     return cudaErrorInvalidValue;
+}
+
+// f16 weights: the epilogue kind is a template parameter.  Quantised weights decoded in the kernel (first-generation launch) take the
+// general epilogue, which recognises the same kinds per value with the same formulas (one instantiation per weight type and tile width)
+template <int WT>
+static cudaError_t launch_ek(const GemmDesc & g, const GemmKParams & kp, bool persistent, cudaStream_t st) {
+    if constexpr (WT != WT_F16) {
+        return launch_bn<WT, EPI_GENERAL>(g, kp, persistent, st);
+    } else {
+        switch (epi_kind(g.ep)) {
+            case EPI_F16:        return launch_bn<WT, EPI_F16>(g, kp, persistent, st);
+            case EPI_F16_GELU:   return launch_bn<WT, EPI_F16_GELU>(g, kp, persistent, st);
+            case EPI_F32_RES:    return launch_bn<WT, EPI_F32_RES>(g, kp, persistent, st);
+            case EPI_F16_MMAJOR: return launch_bn<WT, EPI_F16_MMAJOR>(g, kp, persistent, st);
+            case EPI_F16_HM:     return launch_bn<WT, EPI_F16_HM>(g, kp, persistent, st);
+            case EPI_GENERAL:    return launch_bn<WT, EPI_GENERAL>(g, kp, persistent, st);
+        }
+        return cudaErrorInvalidValue;
+    }
 }
 
 cudaError_t dequant_to_f16(const QMat & W, int64_t rows, __half * out, cudaStream_t st) {
@@ -386,15 +569,15 @@ cudaError_t gemm_launch(const GemmDesc & g, cudaStream_t st) {
     if (g.half_box_b && g.BN < 128) return cudaErrorInvalidValue;
     if (g.v2 && (g.A.type == WT_F16 || g.a16)) {                  // persistent kernel: both operands f16 through TMA
         if (g.A.type != WT_F16 && !g.a16_keep) { const cudaError_t e = dequant_launch(g, st); if (e != cudaSuccess) return e; }
-        return launch_bn<WT_F16>(g, kp, true, st);
+        return launch_ek<WT_F16>(g, kp, true, st);
     }
     switch (g.A.type) {
-        case WT_F16:  return launch_bn<WT_F16>(g, kp, false, st);
-        case WT_Q4_0: return launch_bn<WT_Q4_0>(g, kp, false, st);
-        case WT_Q5_0: return launch_bn<WT_Q5_0>(g, kp, false, st);
-        case WT_Q8_0: return launch_bn<WT_Q8_0>(g, kp, false, st);
-        case WT_Q4_K: return launch_bn<WT_Q4_K>(g, kp, false, st);
-        case WT_Q5_K: return launch_bn<WT_Q5_K>(g, kp, false, st);
+        case WT_F16:  return launch_ek<WT_F16>(g, kp, false, st);
+        case WT_Q4_0: return launch_ek<WT_Q4_0>(g, kp, false, st);
+        case WT_Q5_0: return launch_ek<WT_Q5_0>(g, kp, false, st);
+        case WT_Q8_0: return launch_ek<WT_Q8_0>(g, kp, false, st);
+        case WT_Q4_K: return launch_ek<WT_Q4_K>(g, kp, false, st);
+        case WT_Q5_K: return launch_ek<WT_Q5_K>(g, kp, false, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -39,6 +39,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) { }
 }
 
+// ---------------------------------------------------------------- register reallocation (every warp of a warpgroup executes it)
+template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(N)); }
+template <int N> __device__ __forceinline__ void reg_alloc()   { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(N)); }
+
 // ---------------------------------------------------------------- proxies / fences
 // generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
