@@ -139,7 +139,9 @@ def bind_whisper_api(L):
 class WhisperB200:
     """Minimal object wrapper: one context (weights on `gpu_device`) + its default state."""
 
-    def __init__(self, model_path, gpu_device=0, lib_path=LIB_PATH):
+    def __init__(self, model_path, gpu_device=0, lib_path=LIB_PATH, dtw_aheads_preset=None, dtw_n_top=-1):
+        """dtw_aheads_preset: a whisper_alignment_heads_preset value (1 = the dtw_n_top last layers, 3.. = the tables of the released
+        models) turns on DTW token timestamps (flash_attn off, as whisper.h requires): every text token gets a t_dtw, see tokens()"""
         if not os.path.exists(lib_path):
             raise RuntimeError(f"{lib_path} is missing: build it with __graft_entry__.build() (nvcc, sm_90a); there is no CPU fallback")
         self.L = bind_whisper_api(C.CDLL(lib_path))
@@ -149,6 +151,8 @@ class WhisperB200:
         self.L.wb200_ctx_state.argtypes = [C.c_void_p]
         cp = self.L.whisper_context_default_params()
         cp.gpu_device = gpu_device
+        if dtw_aheads_preset is not None:
+            cp.flash_attn = False; cp.dtw_token_timestamps = True; cp.dtw_aheads_preset = int(dtw_aheads_preset); cp.dtw_n_top = int(dtw_n_top)
         self.ctx = self.L.whisper_init_from_file_with_params(os.fsencode(model_path), cp)
         if not self.ctx:
             raise RuntimeError("whisper_init_from_file_with_params failed: " + self.L.wb200_last_error().decode())
@@ -178,6 +182,12 @@ class WhisperB200:
             out.append((L.whisper_full_get_segment_t0(ctx, i), L.whisper_full_get_segment_t1(ctx, i),
                         L.whisper_full_get_segment_text(ctx, i).decode("utf-8", "replace"), toks))
         return out
+
+    def tokens(self):
+        """per segment, per token: (id, t0, t1, t_dtw) in centiseconds; t_dtw is -1 unless the context has DTW token timestamps"""
+        L, ctx = self.L, self.ctx
+        return [[(t.id, t.t0, t.t1, t.t_dtw) for t in (L.whisper_full_get_token_data(ctx, i, j) for j in range(L.whisper_full_n_tokens(ctx, i)))]
+                for i in range(L.whisper_full_n_segments(ctx))]
 
     def launch_count(self):
         return int(self.L.wb200_launch_count())

@@ -159,61 +159,28 @@ void account_decode(whisper_state & st, int n_tokens, int64_t dt) {             
 } // namespace
 
 bool encode_window(whisper_context & ctx, whisper_state & st, int mel_offset) {
-    const int64_t t0 = time_us();
     const int n_ctx = st.exp_n_audio_ctx > 0 ? st.exp_n_audio_ctx : ctx.model.hp.n_audio_ctx;
 
     if (st.fe.n_mel != ctx.model.hp.n_mels) { set_error("encode: mel has %d bands, model expects %d", st.fe.n_mel, ctx.model.hp.n_mels); return false; }
-    if (st.group) {
-        Group::Req r; r.kind = 0; r.ctx = &ctx; r.st = &st; r.seek = mel_offset; r.n_ctx = n_ctx;
-        if (!st.group->submit(r)) return false;
-        st.t_encode_us += r.dt_us;
-    } else {
-        const EncSrc src = { st.fe.mel.p, st.fe.n_len, st.fe.n_mel, mel_offset, st.slot };
-        if (!st.eng->encode(&src, 1, n_ctx)) return false;
-        st.t_encode_us += time_us() - t0;
-    }
+    if (!st.group) { set_error("encode: the state is not attached to a device pool"); return false; }
+    Group::Req r; r.kind = 0; r.ctx = &ctx; r.st = &st; r.seek = mel_offset; r.n_ctx = n_ctx;
+    if (!st.group->submit(r)) return false;
+    st.t_encode_us += r.dt_us;
     st.n_encode++;
     return true;
 }
 
 bool decode_batch(whisper_context & ctx, whisper_state & st, const int * tokens, const int * pos, const int * seq,
-                  const int8_t * want, int n_tokens, const SampReq * samp) {
-    const int64_t t0 = time_us();
-    const int n_vocab = ctx.model.hp.n_vocab;
+                  const int8_t * want, int n_tokens, const SampReq * samp, int dtw_n_ctx) {
     if (st.scripted) {                                                       // test hook: what was fed to the decoder (wb200_dbg_last_batch)
         st.dbg_tok.assign(tokens, tokens + n_tokens); st.dbg_pos.assign(pos, pos + n_tokens);
         st.dbg_seq.assign(seq, seq + n_tokens); st.dbg_want.assign(want, want + n_tokens);
     }
-    if (st.group) {
-        Group::Req r; r.kind = 1; r.ctx = &ctx; r.st = &st; r.tokens = tokens; r.pos = pos; r.seq = seq; r.want = want; r.n = n_tokens; r.samp = samp;
-        if (!st.group->submit(r)) return false;
-        account_decode(st, n_tokens, r.dt_us);
-        note_rows(ctx, st, want, n_tokens);
-        return true;
-    }
-    PreparedDecode P;
-    if (!prepare_decode(st, tokens, pos, seq, want, n_tokens, P)) return false;
-    if (st.scripted) {                                                       // test hook: KV bookkeeping only, the caller's logits callback supplies the values
-        scripted_attended(st, P, n_tokens);
-        st.samp_out.clear(); st.logits.assign((size_t) n_tokens * n_vocab, 0.0f);
-        account_decode(st, n_tokens, time_us() - t0);
-        note_rows(ctx, st, want, n_tokens);
-        return true;
-    }
-    if (samp) {
-        if (!st.eng->set_samp_mask(samp->mask_key, *samp->mask_bits)) return false;
-        const int stride = samp->draws ? samp->stride : 1;
-        st.samp_stride = stride;
-        st.samp_out.assign((size_t) n_tokens * stride, SampOut());
-        if (!st.eng->decode(P.rows.data(), n_tokens, P.cells.data(), P.idx.data(), P.ld, P.nkv.data(), nullptr, &samp->cfg, samp->rowinfo, st.samp_out.data(), samp->draws, stride)) return false;
-    } else {
-        st.samp_out.clear();
-        st.logits.resize((size_t) n_tokens * n_vocab);
-        std::vector<float *> outs(n_tokens);
-        for (int j = 0; j < n_tokens; ++j) outs[j] = st.logits.data() + (size_t) j * n_vocab;
-        if (!st.eng->decode(P.rows.data(), n_tokens, P.cells.data(), P.idx.data(), P.ld, P.nkv.data(), outs.data())) return false;
-    }
-    account_decode(st, n_tokens, time_us() - t0);
+    if (!st.group) { set_error("decode: the state is not attached to a device pool"); return false; }
+    Group::Req r; r.kind = 1; r.ctx = &ctx; r.st = &st; r.tokens = tokens; r.pos = pos; r.seq = seq; r.want = want; r.n = n_tokens; r.samp = samp;
+    r.dtw_n_ctx = dtw_n_ctx;
+    if (!st.group->submit(r)) return false;
+    account_decode(st, n_tokens, r.dt_us);
     note_rows(ctx, st, want, n_tokens);
     return true;
 }
@@ -242,6 +209,7 @@ bool Group::grow_locked(std::unique_lock<std::mutex> & lk, int new_cap, int new_
     if (!scripted) {
         if (cap == 0) {
             if (!eng.init(model, 1)) return false;                                   // one slot, GGML_PAD(n_text_ctx, 256) cells
+            if (!eng.dtw_set_heads(dtw_heads)) return false;
             cap = 1; cps = eng.cps;
         }
         if ((new_cap != cap || new_cps != cps) && !eng.resize(new_cap, new_cps)) return false;
@@ -428,13 +396,26 @@ void Group::run(std::vector<Req *> & batch) {
             total += q->n; ld = std::max(ld, preps[i].ld);
         }
         // the on-device filter + pick serves the pass only if EVERY request asked for it with the same configuration (a member that fell
-        // back to temperature > 0 samples on the host and needs full logits, so the whole pass returns logits then)
-        bool all_samp = dec[0]->samp != nullptr;
+        // back to temperature > 0 samples on the host and needs full logits, so the whole pass returns logits then).  A DTW pass samples
+        // nothing: the one row it wants needs only the raw summary (max, sum, no-speech logit) of the sampler output, which does not depend
+        // on the filter configuration, so it rides on whatever configuration the other requests share (its own, when it offers one and
+        // only DTW passes are in the batch).
+        const Req * cfg0 = nullptr;
+        for (Req * q : dec) if (!q->dtw_n_ctx) { cfg0 = q; break; }
+        if (!cfg0) for (Req * q : dec) if (q->samp) { cfg0 = q; break; }
+        bool all_samp = cfg0 != nullptr && cfg0->samp != nullptr;
         auto same_cfg = [](const SampCfg & a, const SampCfg & b) {            // field by field: the struct has padding bytes
             return a.token_eot == b.token_eot && a.token_beg == b.token_beg && a.token_nosp == b.token_nosp && a.space_id == b.space_id &&
                    a.suppress_blank == b.suppress_blank && a.no_timestamps == b.no_timestamps && a.max_initial_tid == b.max_initial_tid;
         };
-        for (Req * q : dec) all_samp = all_samp && q->samp != nullptr && q->samp->mask_key == dec[0]->samp->mask_key && same_cfg(q->samp->cfg, dec[0]->samp->cfg);
+        for (Req * q : dec) if (!q->dtw_n_ctx) all_samp = all_samp && q->samp != nullptr && q->samp->mask_key == cfg0->samp->mask_key && same_cfg(q->samp->cfg, cfg0->samp->cfg);
+        // DTW requests: capture indices [cap0, cap0 + n) of the engine's capture buffer, one region per request
+        std::vector<int> dtw_req; std::vector<Req *> dtw_of;
+        int n_cap = 0;
+        for (Req * q : dec) if (q->dtw_n_ctx > 0) {
+            dtw_req.insert(dtw_req.end(), { n_cap, q->st->slot, q->n, q->dtw_n_ctx });
+            dtw_of.push_back(q); n_cap += q->n;
+        }
         if (scripted) {                                               // test hook: KV bookkeeping done above, logits are the callback's business
             for (size_t i = 0; i < dec.size(); ++i) {
                 Req * q = dec[i];
@@ -442,18 +423,22 @@ void Group::run(std::vector<Req *> & batch) {
                 q->st->samp_out.clear(); q->st->logits.assign((size_t) q->n * n_vocab, 0.0f);
             }
         } else {
-        if (ok && all_samp) ok = eng.set_samp_mask(dec[0]->samp->mask_key, *dec[0]->samp->mask_bits);
+        if (ok && all_samp) ok = eng.set_samp_mask(cfg0->samp->mask_key, *cfg0->samp->mask_bits);
+        if (ok && n_cap > 0) ok = eng.dtw_reserve(n_cap);
         if (ok) {
             std::vector<DecToken> rows; std::vector<int> cells, nkv, idx((size_t) total * ld, 0); std::vector<float *> outs;
             int stride = 1;                                            // entries per row of the sampler output: the widest request decides
-            if (all_samp) for (Req * q : dec) stride = std::max(stride, q->samp->draws ? q->samp->stride : 1);
-            std::vector<int> rowinfo; std::vector<SampOut> souts((size_t) total * stride); std::vector<std::pair<Req *, int>> origin;
+            auto own_stride = [](const Req * q) { return (q->samp && q->samp->draws) ? q->samp->stride : 1; };
+            if (all_samp) for (Req * q : dec) stride = std::max(stride, own_stride(q));
+            std::vector<int> rowinfo, capidx; std::vector<SampOut> souts((size_t) total * stride); std::vector<std::pair<Req *, int>> origin;
+            std::vector<int> cap0(dec.size(), -1);
+            for (size_t i = 0, c = 0; i < dec.size(); ++i) if (dec[i]->dtw_n_ctx > 0) { cap0[i] = dtw_req[4 * c]; ++c; }
             std::vector<double> draws; if (stride > 1) draws.assign((size_t) total * stride, 0.0);
             rows.reserve(total);
             // interleave: row k of every request first, so that single-token steps of all members share one pass (<= Engine::max_rows rows)
             // and multi-token prompts advance in lock-step (causal order inside each member is preserved)
             int maxn = 0; for (Req * q : dec) maxn = std::max(maxn, q->n);
-            for (Req * q : dec) { if (all_samp) { q->st->samp_stride = q->samp->draws ? q->samp->stride : 1; q->st->samp_out.assign((size_t) q->n * q->st->samp_stride, SampOut()); } else { q->st->samp_out.clear(); q->st->logits.resize((size_t) q->n * n_vocab); } }
+            for (Req * q : dec) { if (all_samp) { q->st->samp_stride = own_stride(q); q->st->samp_out.assign((size_t) q->n * q->st->samp_stride, SampOut()); } else { q->st->samp_out.clear(); q->st->logits.resize((size_t) q->n * n_vocab); } }
             for (int k = 0; k < maxn; ++k) {
                 for (size_t i = 0; i < dec.size(); ++i) {
                     Req * q = dec[i]; if (k >= q->n) continue;
@@ -462,7 +447,10 @@ void Group::run(std::vector<Req *> & batch) {
                     rows.push_back(P.rows[k]); cells.push_back(P.cells[k]); nkv.push_back(P.nkv[k]);
                     memcpy(idx.data() + r * ld, P.idx.data() + (size_t) k * P.ld, (size_t) P.nkv[k] * sizeof(int));
                     outs.push_back(all_samp ? nullptr : q->st->logits.data() + (size_t) k * n_vocab);
-                    if (all_samp) {
+                    capidx.push_back(cap0[i] >= 0 ? cap0[i] + k : -1);
+                    if (all_samp && q->dtw_n_ctx > 0) {               // DTW row: greedy pick without draws, only its raw summary is read
+                        rowinfo.push_back(0); rowinfo.push_back(0);
+                    } else if (all_samp) {
                         const bool has_draws = q->samp->draws != nullptr;
                         rowinfo.push_back(has_draws ? q->samp->rowinfo[2*k] : (q->samp->rowinfo[2*k] & 0xff)); rowinfo.push_back(q->samp->rowinfo[2*k + 1]);
                         if (has_draws) memcpy(draws.data() + r * stride, q->samp->draws + (size_t) k * q->samp->stride, (size_t) q->samp->stride * sizeof(double));
@@ -471,14 +459,22 @@ void Group::run(std::vector<Req *> & batch) {
                 }
             }
             if (all_samp) {
-                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), nullptr, &dec[0]->samp->cfg, rowinfo.data(), souts.data(),
-                                stride > 1 ? draws.data() : nullptr, stride);
+                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), nullptr, &cfg0->samp->cfg, rowinfo.data(), souts.data(),
+                                stride > 1 ? draws.data() : nullptr, stride, n_cap > 0 ? capidx.data() : nullptr);
                 for (int r = 0; r < total; ++r) {
-                    Req * q = origin[r].first; const int own = q->samp->draws ? q->samp->stride : 1;
+                    Req * q = origin[r].first; const int own = own_stride(q);
                     for (int j = 0; j < own; ++j) q->st->samp_out[(size_t) origin[r].second * own + j] = souts[(size_t) r * stride + j];
                 }
             } else {
-                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), outs.data());
+                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), outs.data(), nullptr, nullptr, nullptr, nullptr, 1,
+                                n_cap > 0 ? capidx.data() : nullptr);
+            }
+            // alignment weights of every DTW request of the batch in one launch (the host DTW runs on each state's own thread)
+            if (ok && n_cap > 0) {
+                std::vector<std::vector<float> *> outw;
+                for (Req * q : dtw_of) outw.push_back(&q->st->dtw_qk_last);
+                ok = eng.dtw_weights(dtw_req, outw);
+                for (Req * q : dtw_of) { whisper_state & s = *q->st; s.dtw_last_shape[0] = q->n; s.dtw_last_shape[1] = q->dtw_n_ctx; s.dtw_last_shape[2] = eng.dtw_n_heads; }
             }
         }
         }
@@ -558,9 +554,6 @@ WB_EXPORT struct whisper_context * whisper_init_with_params_no_state(struct whis
                 ctx = new whisper_context();
                 ctx->params = params;
                 ctx->t_start_us = time_us();
-                // DTW token timestamps need the cross-attention queries layer by layer: such a context keeps the decoder weights planar and
-                // decodes with the kernel-per-op chain (the persistent kernel never materialises them)
-                ctx->model.force_planar = params.dtw_token_timestamps;
                 ok = model_load(loader, ctx->model, ctx->vocab, params.gpu_device);
                 ctx->t_load_us = ctx->model.t_load_us;
             }
@@ -637,23 +630,12 @@ WB_EXPORT struct whisper_state * whisper_init_state(struct whisper_context * ctx
         logf(LOG_INFO, "%s: alignment heads masks: %d heads\n", __func__, (int) ctx->dtw_heads.size());
     }
     try {
-        if (ctx->params.dtw_token_timestamps && !ctx->scripted) {
-            // DTW contexts decode with the kernel-per-op chain and capture queries layer by layer: a private engine per state, no pool
-            st = new whisper_state();
-            st->own_eng.reset(new Engine());
-            st->eng = st->own_eng.get();
-            if (!st->fe.init(&ctx->model) || !st->eng->init(&ctx->model, 1)) { delete st; return nullptr; }
-            st->kv.reset((uint32_t) st->eng->n_cells);
-            st->kv_self_n_dec = 1;
-            st->decoders[0].rng = std::mt19937(0);
-            return st;
-        }
-        // every other state is a slot of a device pool of the context (created with the first state); see wb_state.h.  With replicas on
+        // every state is a slot of a device pool of the context (created with the first state); see wb_state.h.  With replicas on
         // several GPUs the new state goes to the GPU that holds the fewest states (ties: the context's own device first).
         Group * pool = nullptr; const Model * model = &ctx->model;
         {
             std::lock_guard<std::mutex> lk(ctx->replicas_mu);
-            if (!ctx->pool) { ctx->pool.reset(new Group()); ctx->pool->model = &ctx->model; ctx->pool->scripted = ctx->scripted; }
+            if (!ctx->pool) { ctx->pool.reset(new Group()); ctx->pool->model = &ctx->model; ctx->pool->scripted = ctx->scripted; ctx->pool->dtw_heads = ctx->dtw_heads; }
             pool = ctx->pool.get();
             for (auto & r : ctx->replicas) {
                 if (!r->pool) { r->pool.reset(new Group()); r->pool->model = &r->model; }

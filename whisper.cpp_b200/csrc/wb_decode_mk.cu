@@ -24,6 +24,7 @@
 #include <cmath>
 #include <type_traits>
 #include "wb_decode_mk.cuh"
+#include "wb_dtw_kernel.cuh"
 #include "wb_common.h"
 #include "wb_dev.cuh"
 #include "wb_ptx.cuh"
@@ -966,6 +967,11 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) 
     asm volatile("cp.async.wait_all;" ::: "memory");
 }
 
+// DTW: copy the alignment-head slices of the cross-Q rows (complete after the barrier that ended phase 6) into the capture buffer
+__device__ __noinline__ void mk_dtw_capture(const MkArgs & a, const MkLayer & L) {
+    dtw_capture_rows(a.q2, a.d, a.cap_row, a.n_tok, L.cap_mask, L.cap_head0, a.cap, a.cap_rows, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
+}
+
 #define MK_SYNC() do { MK_STAMP(); target += gridDim.x; mk_grid_sync(a, target); MK_STAMP(); } while (0)
 #define MK_SYNC_Q() do { target += gridDim.x; mk_grid_sync(a, target); } while (0)      // without trace stamps (24 per layer for every format)
 
@@ -1010,8 +1016,9 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
         e = MkEpi(); e.bias = L.cq_bias; e.out = a.q2;
         mk_gemv<WT, false>(a, L.cq, a.actq, e, (TRACE && l == 1) ? 2048 + 16 : -1);
         MK_SYNC();
-        // 7: cross-attention (2688-2705)
+        // 7: cross-attention (2688-2705); DTW passes first keep the alignment-head queries of their flagged rows
         if (pf_w) mk_prefetch_w(L.fc2);
+        if (a.cap != nullptr && L.cap_mask != 0u) mk_dtw_capture(a, L);
         mk_attn_cross<WT>(a, L);
         if (mk_kq(WT)) { MK_SYNC_Q(); mk_q8k_rows(a, a.qkv, d, a.actq); }
         MK_SYNC();

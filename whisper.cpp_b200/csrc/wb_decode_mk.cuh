@@ -15,6 +15,7 @@ struct MkLayer {                      // one text layer: weights (model) + this 
     const float * qkv_bias, * qkv_scale, * o_bias, * cq_bias, * co_bias, * fc1_bias, * fc2_bias;
     __half * kc, * vc;                // self-attention KV of this layer: [n_cells][d]
     const __half * xk, * xv;          // cross-attention K / V of this layer in slot 0: [Tp][d]
+    uint32_t cap_mask; int cap_head0; // DTW: alignment heads of this layer (bit h = head h) and the capture head of the lowest (wb_dtw_kernel.cuh)
 };
 
 struct MkArgs {
@@ -33,6 +34,7 @@ struct MkArgs {
     unsigned long long bar_base;      // its value when this launch starts
     int * err;                        // set to 1 when a barrier wait times out
     long long * trace;                // optional: phase time stamps of CTA 0 (see MK_STAMP)
+    float * cap = nullptr; const int * cap_row = nullptr; int cap_rows = 0;   // DTW capture (generation 1 only): null when no row of the pass has a capture index
     int prefetch;                     // bit0: next-phase weights -> L2, bit1: cross KV -> L2 one phase ahead
     // second generation (wb_decode_mk2.cu) only:
     int global_sync = 0;              // a row attends to self-KV cells another row GROUP writes in this pass: all groups meet after the KV append

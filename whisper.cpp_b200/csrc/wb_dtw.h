@@ -1,6 +1,6 @@
 // wb_dtw.h -- DTW token timestamps (whisper_context_params.dtw_token_timestamps; src/whisper.cpp:8856-9167).
-// The cross-attention weights of the alignment heads come from the device (wb_engine: one extra decoder pass over the window's text with
-// the kernel-per-op chain, k_dtw_qk); everything after that -- normalisation over the tokens, 7-tap median filter over time, mean over
+// The cross-attention weights of the alignment heads come from the device (one extra decoder pass over the window's text, batched with the
+// other states of the pool, whose rows capture the alignment-head queries; k_dtw_qk); everything after that -- normalisation over the tokens, 7-tap median filter over time, mean over
 // heads, dynamic time warping, backtrace, assignment to tokens -- is host code here.
 #pragma once
 #include <cstdint>

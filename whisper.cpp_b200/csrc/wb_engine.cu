@@ -150,7 +150,7 @@ bool Engine::set_cells(int n) {
     const size_t e = (size_t) hp.n_text_layer * n * hp.n_text_state;
     if (!kv_k.alloc(e, true) || !kv_v.alloc(e, true)) return false;
     ld_idx = pad256(hp.n_text_ctx);          // a query attends to at most n_text_ctx positions
-    const size_t nints = (size_t) max_rows * (7 + ld_idx);
+    const size_t nints = (size_t) max_rows * (8 + ld_idx);
     if (!dints.alloc(nints)) return false;
     if (hints) cudaFreeHost(hints);
     hints = nullptr;
@@ -227,6 +227,7 @@ bool Engine::mk_build_table() {
         t.fc1_bias = L.fc1_bias; t.fc2_bias = L.fc2_bias;
         t.kc = kv_k.p + (size_t) l * n_cells * d; t.vc = kv_v.p + (size_t) l * n_cells * d;
         t.xk = kv_cross.p + (size_t) l * Tp * d;  t.xv = kv_cross.p + (size_t) (Lt + l) * Tp * d;
+        t.cap_mask = dtw_layer_mask.empty() ? 0u : dtw_layer_mask[l]; t.cap_head0 = dtw_layer_head0.empty() ? 0 : dtw_layer_head0[l];
     }
     if (!mk_layers.alloc(Lt)) return false;
     WB_CUDA_OK(cudaMemcpy(mk_layers.p, tab.data(), Lt * sizeof(MkLayer), cudaMemcpyHostToDevice));
@@ -470,9 +471,10 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
     const int Tp = Tp_max;                                         // kv_cross layout stride
     const float kq_scale = powf(64.0f, -0.25f);                    // whisper.cpp:2514
     const int R = max_rows;
-    const size_t nint = (size_t) 7 * R + (size_t) n * ld_idx;          // packed: tok | pos | cell | slot | n_kv | rowinfo[2] | idx rows
+    const size_t nint = (size_t) 8 * R + (size_t) n * ld_idx;          // packed: tok | pos | cell | slot | n_kv | rowinfo[2] | capture index | idx rows
     WB_CUDA_OK(cudaMemcpyAsync(dints.p, hints, nint * sizeof(int), cudaMemcpyHostToDevice, st));
-    const int * d_tok = dints.p, * d_pos = dints.p + R, * d_cell = dints.p + 2 * R, * d_slot = dints.p + 3 * R, * d_nkv = dints.p + 4 * R, * d_row = dints.p + 5 * R, * d_idx = dints.p + 7 * R;
+    const int * d_tok = dints.p, * d_pos = dints.p + R, * d_cell = dints.p + 2 * R, * d_slot = dints.p + 3 * R, * d_nkv = dints.p + 4 * R, * d_row = dints.p + 5 * R;
+    const int * d_cap = dints.p + 7 * R, * d_idx = dints.p + 8 * R;
 
     dec_embed(m->d_te, m->d_pe, d_tok, d_pos, n, d, dx.p, st);
     if (use_mk) {
@@ -485,15 +487,22 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         a.x = dx.p; a.qkv = dqkv.p; a.q2 = dq2.p; a.logits = dlogits.p;
         a.actq = reinterpret_cast<uint8_t *>(dattn.p); a.h = dh.p; a.hq = dhq.p;
         a.xpart = xpart.p; a.xcnt = xcnt.p;
+        if (pass_capture) { a.cap = dtw_q.p; a.cap_row = d_cap; a.cap_rows = dtw_cap_rows; }
+        const int gen = (mk_gen == 2 && !pass_capture) ? 2 : 1;      // DTW capture exists in generation 1 only
+        if (mk_last_gen != 0 && gen != mk_last_gen) {                // the generations lay their barrier words out differently: start from zero
+            WB_CUDA_OK(cudaMemsetAsync(mk_bar.p, 0, mk_bar.bytes(), st));
+            mk_bar_total = 0;
+        }
+        mk_last_gen = gen;
         a.bar = mk_bar.p; a.bar_base = mk_bar_total; a.err = reinterpret_cast<int *>(mk_bar.p + 8); a.prefetch = mk_prefetch; a.trace = mk_trace.p;
-        if (mk_gen == 2) {
+        if (gen == 2) {
             // does a row attend to a self-KV cell that a row of ANOTHER 16-row group appends in this pass (several tokens of one sequence)?
             a.stagger_clk = mk_stagger_clk;
             if (n > 16) {
                 if (cell_group.size() < (size_t) n_cells) cell_group.assign(n_cells, 0);
                 ++cell_stamp;
                 if ((cell_stamp & 0xffffff) == 0) { std::fill(cell_group.begin(), cell_group.end(), 0u); cell_stamp = 1; }
-                const int * h_cell = hints + 2 * R, * h_nkv = hints + 4 * R, * h_idx = hints + 7 * R;
+                const int * h_cell = hints + 2 * R, * h_nkv = hints + 4 * R, * h_idx = hints + 8 * R;
                 for (int t = 0; t < n; ++t) cell_group[h_cell[t]] = (cell_stamp << 8) | (uint32_t) (t >> 4);
                 for (int t = 0; t < n && !a.global_sync; ++t) {
                     const int * row = h_idx + (size_t) t * ld_idx;
@@ -515,7 +524,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         for (int j = 0; j < n; ++j) kvbytes += (double) Lt * 2.0 * d * 2.0 * ((double) n_keys + hints[4 * R + j]);
         flops += kvbytes;                                           // 2 flops per KV element (f16 = 2 bytes): same number
         ProfScope prof(PC_GEMV, st, wbytes + kvbytes, flops);
-        if (mk_gen == 2) {
+        if (gen == 2) {
             if (!mk2_launch(a, m->wtype == WT_F32 ? WT_F16 : m->wtype, n_sm, st)) return false;
             mk_bar_total += 4096;
         } else {
@@ -534,8 +543,8 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         { GemvArgs a; a.W = L.o; a.x = dattn.p; a.n_tok = n; a.bias = L.o_bias; a.res = dx.p; a.out = dx.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }    // 2647-2659
         { GemvArgs a; a.W = L.cq; a.x = dx.p; a.n_tok = n; a.ln_w = L.lnc.w; a.ln_b = L.lnc.b; a.eps = hp.eps;        // 2661-2681
           a.bias = L.cq_bias; a.out = dq2.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }
-        if (dtw_cap.active && dtw_cap.layer_slot[l] >= 0)            // DTW pass: keep this layer's cross-attention queries of the rows of this pass
-            WB_CUDA_OK(cudaMemcpyAsync(dtw_q.p + ((size_t) dtw_cap.layer_slot[l] * dtw_cap.n_total + dtw_cap.row0) * d, dq2.p, (size_t) n * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (pass_capture && dtw_layer_mask[l] != 0u &&               // DTW rows: keep the alignment-head queries of this layer
+            !dtw_capture_launch(dq2.p, d, d_cap, n, dtw_layer_mask[l], dtw_layer_head0[l], dtw_q.p, dtw_cap_rows, st)) return false;
         attn_cross_decode(dq2.p, d, kv_cross.p + (size_t) l * Tp * d, kv_cross.p + (size_t) (Lt + l) * Tp * d, d_slot,
                           (int64_t) 2 * Lt * Tp * d, n_keys, n, H, d, kq_scale, xpart.p, xcnt.p, dattn.p, d, st);       // 2688-2705
         { GemvArgs a; a.W = L.co; a.x = dattn.p; a.n_tok = n; a.bias = L.co_bias; a.res = dx.p; a.out = dx.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }  // 2754-2766
@@ -559,7 +568,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
 }
 
 bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, float * const * logits_out,
-                    const SampCfg * samp, const int * rowinfo, SampOut * samp_out, const double * draws, int stride) {
+                    const SampCfg * samp, const int * rowinfo, SampOut * samp_out, const double * draws, int stride, const int * cap_idx) {
     NvtxRange nvtx("wb200.decode");
     const HParams & hp = m->hp;
     WB_CUDA_OK(cudaSetDevice(m->device));
@@ -570,8 +579,10 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
     const int R = max_rows;
     for (int r0 = 0; r0 < n_rows; r0 += R) {
         const int n = std::min(R, n_rows - r0);
-        int * h_tok = hints, * h_pos = hints + R, * h_cell = hints + 2 * R, * h_slot = hints + 3 * R, * h_nkv = hints + 4 * R, * h_row = hints + 5 * R, * h_idx = hints + 7 * R;
+        int * h_tok = hints, * h_pos = hints + R, * h_cell = hints + 2 * R, * h_slot = hints + 3 * R, * h_nkv = hints + 4 * R, * h_row = hints + 5 * R;
+        int * h_cap = hints + 7 * R, * h_idx = hints + 8 * R;
         bool any_logits = false;
+        pass_capture = false;
         for (int j = 0; j < n; ++j) {
             const DecToken & t = rows[r0 + j];
             if (t.token < 0 || t.token >= V || t.pos < 0 || t.pos >= hp.n_text_ctx || t.slot < 0 || t.slot >= cap_win) {
@@ -581,6 +592,9 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
             h_tok[j] = t.token; h_pos[j] = t.pos; h_cell[j] = cells[r0 + j]; h_slot[j] = t.slot; h_nkv[j] = n_kv[r0 + j];
             h_row[2*j] = (samp && rowinfo) ? rowinfo[2*(r0 + j)] : 0; h_row[2*j + 1] = (samp && rowinfo) ? rowinfo[2*(r0 + j) + 1] : 0;
             memcpy(h_idx + (size_t) j * ld_idx, kv_idx + (size_t) (r0 + j) * ld, (size_t) n_kv[r0 + j] * sizeof(int));
+            h_cap[j] = cap_idx ? cap_idx[r0 + j] : -1;
+            if (h_cap[j] >= dtw_cap_rows) { set_error("decode: capture index %d exceeds the capture buffer (%d rows)", h_cap[j], dtw_cap_rows); return false; }
+            pass_capture |= h_cap[j] >= 0;
             any_logits |= t.want_logits;
         }
         draw_stride = (samp && draws && stride > 1) ? std::min(stride, (int) SAMP_MAX_DRAWS) : 1;
@@ -591,15 +605,14 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
         } else {
             for (int j = 0; j < n; ++j) h_row[2*j] &= 0xff;           // no uniforms supplied: greedy picks only
         }
-        count_h2d(((size_t) 7 * R + (size_t) n * ld_idx) * sizeof(int));
+        count_h2d(((size_t) 8 * R + (size_t) n * ld_idx) * sizeof(int));
         if (any_logits) count_d2h(samp ? (uint64_t) n * draw_stride * sizeof(SampOut) : (uint64_t) n * V * 4);
 
         // One pass = 8 kernels per text layer.  After the second use of a shape the chain is replayed as a CUDA graph
         // (all per-step values live in `dints`, so kernel arguments never change between steps).
         uint64_t key = (uint64_t) (n | (any_logits ? 128 : 0) | (samp ? 256 : 0)) | ((uint64_t) n_keys << 10) | ((uint64_t) draw_stride << 24);
         if (samp) key |= (uint64_t) ((uint32_t) (samp->token_eot * 31 + samp->token_beg * 17 + samp->token_nosp * 13 + samp->space_id * 7 + samp->max_initial_tid * 3 + samp->no_timestamps * 2 + samp->suppress_blank)) << 32;
-        StepGraph * sg = (use_graphs && !use_mk && !prof_enabled() && !dtw_cap.active) ? &graphs[key] : nullptr;
-        dtw_cap.row0 = r0;
+        StepGraph * sg = (use_graphs && !use_mk && !prof_enabled() && !pass_capture) ? &graphs[key] : nullptr;
         WB_CUDA_OK(cudaEventRecord(ev[5], st));
         if (sg && sg->exec) {
             WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
@@ -641,41 +654,78 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
 
 namespace wb {
 // ---------------------------------------------------------------------------------------------------- DTW capture
-bool Engine::dtw_begin(const std::vector<std::pair<int, int>> & heads, int n_tokens) {
+bool Engine::dtw_set_heads(const std::vector<std::pair<int, int>> & heads) {
     const HParams & hp = m->hp;
-    if (use_mk) { set_error("dtw: this context decodes with the persistent kernel; DTW needs a context created with dtw_token_timestamps"); return false; }
+    const int Lt = hp.n_text_layer, H = hp.n_text_head;
+    if (heads.empty()) return true;
+    if (H > 32) { set_error("dtw: %d heads per layer, the capture takes at most 32", H); return false; }
+    dtw_layer_mask.assign((size_t) Lt, 0u);
+    for (const auto & lh : heads) {
+        if (lh.first < 0 || lh.first >= Lt || lh.second < 0 || lh.second >= H) { set_error("dtw: alignment head (%d, %d) out of range", lh.first, lh.second); return false; }
+        dtw_layer_mask[(size_t) lh.first] |= 1u << lh.second;
+    }
+    dtw_layer_head0.assign((size_t) Lt, 0);
+    for (int l = 1; l < Lt; ++l) dtw_layer_head0[(size_t) l] = dtw_layer_head0[(size_t) l - 1] + __builtin_popcount(dtw_layer_mask[(size_t) l - 1]);
+    dtw_n_heads = (int) heads.size();
+    std::vector<int> tab((size_t) 3 * dtw_n_heads);                   // per alignment head: capture head | layer | head
+    for (int e = 0; e < dtw_n_heads; ++e) {
+        const int l = heads[(size_t) e].first, h = heads[(size_t) e].second;
+        tab[(size_t) e] = dtw_layer_head0[(size_t) l] + __builtin_popcount(dtw_layer_mask[(size_t) l] & ((1u << h) - 1u));
+        tab[(size_t) dtw_n_heads + e] = l; tab[(size_t) 2 * dtw_n_heads + e] = h;
+    }
     WB_CUDA_OK(cudaSetDevice(m->device));
-    dtw_cap.layer_slot.assign((size_t) hp.n_text_layer, -1);
-    dtw_cap.n_sel = 0;
-    for (const auto & lh : heads) if (dtw_cap.layer_slot[(size_t) lh.first] < 0) dtw_cap.layer_slot[(size_t) lh.first] = dtw_cap.n_sel++;
-    dtw_cap.n_total = n_tokens; dtw_cap.row0 = 0;
-    const size_t need = (size_t) dtw_cap.n_sel * n_tokens * hp.n_text_state;
-    if (need > dtw_q.n && !dtw_q.alloc(need)) return false;
-    dtw_cap.active = true;
+    if (!dtw_heads_dev.alloc(tab.size())) return false;
+    WB_CUDA_OK(cudaMemcpy(dtw_heads_dev.p, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+    return !use_mk || mk_build_table();
+}
+
+bool Engine::dtw_reserve(int n_rows) {
+    if (n_rows <= dtw_cap_rows) return true;
+    const int n_cap = dtw_layer_head0.empty() ? 0 : dtw_layer_head0.back() + __builtin_popcount(dtw_layer_mask.back());
+    if (n_cap == 0) { set_error("dtw: the engine has no alignment heads"); return false; }
+    WB_CUDA_OK(cudaSetDevice(m->device));
+    WB_CUDA_OK(cudaStreamSynchronize(st));
+    if (!dtw_q.alloc((size_t) n_cap * n_rows * 64)) return false;
+    dtw_cap_rows = n_rows;
     return true;
 }
-bool Engine::dtw_finish(const std::vector<std::pair<int, int>> & heads, int slot, int n_audio_ctx, std::vector<float> & qk) {
+
+bool Engine::dtw_weights(const std::vector<int> & req, std::vector<std::vector<float> *> & out) {
     const HParams & hp = m->hp;
-    dtw_cap.active = false;
+    const int n_req = (int) req.size() / 4, d = hp.n_text_state, Lt = hp.n_text_layer;
     WB_CUDA_OK(cudaSetDevice(m->device));
-    const int nh = (int) heads.size(), n = dtw_cap.n_total, d = hp.n_text_state, Lt = hp.n_text_layer;
-    std::vector<int> idx((size_t) 3 * nh);
-    for (int e = 0; e < nh; ++e) { idx[(size_t) e] = dtw_cap.layer_slot[(size_t) heads[(size_t) e].first]; idx[(size_t) nh + e] = heads[(size_t) e].first; idx[(size_t) 2 * nh + e] = heads[(size_t) e].second; }
-    if ((size_t) 3 * nh > dtw_idx.n && !dtw_idx.alloc((size_t) 3 * nh)) return false;
-    const size_t n_out = (size_t) nh * n_audio_ctx * n;
-    if (n_out > dtw_out.n && !dtw_out.alloc(n_out)) return false;
-    WB_CUDA_OK(cudaMemcpyAsync(dtw_idx.p, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    std::vector<int64_t> off((size_t) n_req + 1, 0);
+    int max_tokens = 0;
+    for (int r = 0; r < n_req; ++r) {
+        off[(size_t) r + 1] = off[(size_t) r] + (int64_t) dtw_n_heads * req[4 * r + 3] * req[4 * r + 2];
+        max_tokens = std::max(max_tokens, req[4 * r + 2]);
+    }
+    if ((size_t) off.back() > dtw_out.n && !dtw_out.alloc((size_t) off.back())) return false;
+    if (req.size() > dtw_req_dev.n && !dtw_req_dev.alloc(req.size())) return false;
+    if ((size_t) n_req > dtw_req_out.n && !dtw_req_out.alloc((size_t) n_req)) return false;
+    WB_CUDA_OK(cudaMemcpyAsync(dtw_req_dev.p, req.data(), req.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA_OK(cudaMemcpyAsync(dtw_req_out.p, off.data(), (size_t) n_req * sizeof(int64_t), cudaMemcpyHostToDevice, st));
     DtwQkArgs a;
-    a.q = dtw_q.p;
-    a.k_cross = kv_cross.p + (size_t) slot * 2 * Lt * Tp_max * d;        // K part of this slot: [Lt][Tp][d]
-    a.layer_stride = (int64_t) Tp_max * d;
-    a.head_layer_slot = dtw_idx.p; a.head_layer = dtw_idx.p + nh; a.head_index = dtw_idx.p + 2 * nh;
-    a.n_heads = nh; a.n_tokens = n; a.n_audio_ctx = n_audio_ctx; a.d = d; a.scale = powf(64.0f, -0.25f); a.out = dtw_out.p;
+    a.q = dtw_q.p; a.cap_rows = dtw_cap_rows;
+    a.k_cross = kv_cross.p; a.slot_stride = (int64_t) 2 * Lt * Tp_max * d; a.layer_stride = (int64_t) Tp_max * d;   // K part of each slot: [Lt][Tp][d]
+    a.k_head_major = (use_mk && mk_cross_head_major()) ? 1 : 0; a.Tp = Tp_max;
+    a.head_cap = dtw_heads_dev.p; a.head_layer = dtw_heads_dev.p + dtw_n_heads; a.head_index = dtw_heads_dev.p + 2 * dtw_n_heads;
+    a.req = dtw_req_dev.p; a.req_out = dtw_req_out.p;
+    a.n_heads = dtw_n_heads; a.n_req = n_req; a.max_tokens = max_tokens; a.d = d; a.scale = powf(64.0f, -0.25f); a.out = dtw_out.p;
+    for (int r = 0; r < n_req; ++r)
+        if (req[4 * r + 3] <= 0 || req[4 * r + 3] > std::min(Tp_max, 1536) ||   // 1536: the score row of k_dtw_qk in shared memory
+             req[4 * r] < 0 || req[4 * r] + req[4 * r + 2] > dtw_cap_rows) { set_error("dtw: bad request %d", r); return false; }
+    WB_CUDA_OK(cudaEventRecord(ev[5], st));
     if (!dtw_qk_launch(a, st)) return false;
-    qk.resize(n_out);
-    WB_CUDA_OK(cudaMemcpyAsync(qk.data(), dtw_out.p, n_out * sizeof(float), cudaMemcpyDeviceToHost, st));
+    WB_CUDA_OK(cudaEventRecord(ev[6], st));
+    for (int r = 0; r < n_req; ++r) {
+        std::vector<float> & o = *out[(size_t) r];
+        o.resize((size_t) (off[(size_t) r + 1] - off[(size_t) r]));
+        WB_CUDA_OK(cudaMemcpyAsync(o.data(), dtw_out.p + off[(size_t) r], o.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    }
     WB_CUDA_OK(cudaStreamSynchronize(st));
-    count_d2h(n_out * sizeof(float));
+    count_d2h((uint64_t) off.back() * sizeof(float));
+    { float ms = 0.0f; cudaEventElapsedTime(&ms, ev[5], ev[6]); counter_add(8, ms); counter_add(9, n_req); }
     return true;
 }
 } // namespace wb

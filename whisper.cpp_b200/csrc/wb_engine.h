@@ -68,11 +68,18 @@ struct Engine {
     DevBuf<uint8_t> act_scratch;      // quantised activations of the current GEMV (k_act_quant -> k_gemv_mma)
     bool gemv_v2 = true;             // WB200_GEMV_V1=1 selects the dp4a kernel
     // persistent decode kernel (wb_decode_mk.cu); WB200_MEGAKERNEL=0 selects the kernel-per-op chain
-    // DTW token timestamps: while `dtw_cap.active` every chain pass copies the cross-attention queries of the selected layers aside
-    struct DtwCapture { bool active = false; std::vector<int> layer_slot; int n_sel = 0, n_total = 0, row0 = 0; } dtw_cap;
-    DevBuf<float> dtw_q, dtw_out; DevBuf<int> dtw_idx;
-    bool dtw_begin(const std::vector<std::pair<int, int>> & heads, int n_tokens);
-    bool dtw_finish(const std::vector<std::pair<int, int>> & heads, int slot, int n_audio_ctx, std::vector<float> & qk);
+    // DTW token timestamps (wb_dtw_kernel.cuh): a decode row with a capture index >= 0 leaves the cross-attention queries of the alignment
+    // heads in dtw_q [capture head][capture index][64].  Capture heads are the distinct alignment heads ordered by (layer, head).
+    std::vector<uint32_t> dtw_layer_mask;   // per text layer: bit h = head h is an alignment head
+    std::vector<int> dtw_layer_head0;       // per text layer: capture head of its lowest alignment head
+    int dtw_n_heads = 0, dtw_cap_rows = 0;  // alignment heads of the context; rows dtw_q holds per capture head
+    DevBuf<float> dtw_q, dtw_out; DevBuf<int> dtw_heads_dev, dtw_req_dev; DevBuf<int64_t> dtw_req_out;
+    bool pass_capture = false;              // the current pass has rows with a capture index (chain: k_dtw_capture; persistent kernel: generation 1)
+    bool dtw_set_heads(const std::vector<std::pair<int, int>> & heads);   // (text layer, head) in the context's order; once, before any pass
+    bool dtw_reserve(int n_rows);
+    // alignment weights of several DTW passes in one launch: req = 4 ints per request (first capture index, slot, tokens, audio positions);
+    // out[r] receives [heads][audio positions][tokens] of request r
+    bool dtw_weights(const std::vector<int> & req, std::vector<std::vector<float> *> & out);
     bool use_mk = false;
     int  max_rows = 8;               // rows per decode pass: 64 with the persistent kernel, 8 with the chain
     int  n_sm = 0, mk_prefetch = 61;     // bit0: next-phase weights -> L2; bit2: K / V streams with L2 evict-first priority; bit3 (generation 2): row groups take turns in the cross-attention; bit4: logits one warp per weight tile
@@ -87,7 +94,8 @@ struct Engine {
     std::vector<long long> mk_gtrace;
     void mk_trace_collect(int n_layer, bool logits);
     void mk_trace_dump();
-    DevBuf<int>    dints, xcnt;      // packed per-step integers: tokens | pos | cells | slot | n_kv | rowinfo[16] | idx[...]
+    int mk_last_gen = 0;             // generation of the last launch: the two keep different barrier words (reset when they alternate)
+    DevBuf<int>    dints, xcnt;      // packed per-step integers: tokens | pos | cells | slot | n_kv | rowinfo[2] | capture index | idx[...]
     DevBuf<uint32_t> samp_mask;      // static suppression bit mask of the on-device sampler
     uint64_t samp_mask_key = 0;
     DevBuf<SampOut> dsamp;           // [max_rows][SAMP_MAX_DRAWS]
@@ -126,7 +134,8 @@ struct Engine {
     // samp != nullptr: logits stay on the device; the filter + greedy pick run there (rowinfo: 2 ints per row, samp_out: host [n_rows])
     bool decode(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, float * const * logits_out,
                 const SampCfg * samp = nullptr, const int * rowinfo = nullptr, SampOut * samp_out = nullptr,
-                const double * draws = nullptr, int stride = 1);   // draws: [n_rows][stride] uniforms (rows asking for categorical draws, rowinfo bits 8-14); samp_out: [n_rows][stride]
+                const double * draws = nullptr, int stride = 1,    // draws: [n_rows][stride] uniforms (rows asking for categorical draws, rowinfo bits 8-14); samp_out: [n_rows][stride]
+                const int * cap_idx = nullptr);                    // per row: DTW capture index or -1 (null: no row is captured)
     bool set_samp_mask(uint64_t key, const std::vector<uint32_t> & bits);
 };
 

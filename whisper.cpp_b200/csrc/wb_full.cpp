@@ -454,12 +454,12 @@ template <typename F> void run_parallel(int n_threads, F && fn) {
 }
 
 
-// One extra decoder pass over [sot, (lang), no_timestamps, text tokens of the window's segments, eot] with the cross-attention queries of the
-// alignment-head layers captured, their softmax weights over the audio computed on the device, then the host DTW (wb_dtw.cpp).
+// One extra decoder pass over [sot, (lang), no_timestamps, text tokens of the window's segments, eot].  It is an ordinary decode request of the
+// pool that also captures the cross-attention queries of the alignment heads; the batch it joins computes the softmax weights of every
+// DTW request on the device in one launch (Group::run), then the host DTW (wb_dtw.cpp) runs here, on the state's own thread.
 bool dtw_window(whisper_context & ctx, whisper_state & st, const whisper_full_params & params, int i_segment, int n_segments, int seek, int n_frames) {
     const Vocab & vocab = ctx.vocab;
     const int n_audio_ctx = st.exp_n_audio_ctx > 0 ? st.exp_n_audio_ctx : ctx.model.hp.n_audio_ctx;
-    if (st.group || !st.eng) { set_error("dtw: not available for the members of a lock-step batch"); return false; }
     if (n_frames > 2 * n_audio_ctx) { set_error("dtw: %d frames exceed the audio context", n_frames); return false; }
     std::vector<int> tokens = { vocab.token_sot };
     if (vocab.is_multilingual()) { const int lang_id = whisper_lang_id(params.language); st.lang_id = lang_id; tokens.push_back(vocab.token_sot + 1 + lang_id); }
@@ -474,14 +474,22 @@ bool dtw_window(whisper_context & ctx, whisper_state & st, const whisper_full_pa
     want[(size_t) n - 1] = 1;
     st.kv.clear();
     st.kv.seq_rm(0, 0, -1);
-    if (!st.eng->dtw_begin(ctx.dtw_heads, n)) return false;
-    const bool ok = decode_batch(ctx, st, tokens.data(), pos.data(), seq.data(), want.data(), n);
-    if (!ok) { st.eng->dtw_cap.active = false; return false; }
-    if (!st.eng->dtw_finish(ctx.dtw_heads, st.slot, n_audio_ctx, st.dtw_qk_last)) return false;
-    st.dtw_last_shape[0] = n; st.dtw_last_shape[1] = n_audio_ctx; st.dtw_last_shape[2] = (int) ctx.dtw_heads.size();
+    // where the window's own steps use the device sampler, the pass offers the same configuration: a batch of DTW passes alone then still
+    // returns the raw summary of its logits rows instead of full logits
+    std::vector<uint32_t> mask_bits; SampReq sreq; std::vector<int> rowinfo((size_t) 2 * n, 0);
+    const bool dev = !params.logits_filter_callback && !(params.grammar_rules && params.n_grammar_rules > 0) && getenv("WB200_HOST_SAMPLER") == nullptr;
+    if (dev) {
+        build_static_mask(ctx, params, mask_bits, sreq.mask_key);
+        sreq.mask_bits = &mask_bits; sreq.rowinfo = rowinfo.data();
+        make_samp_cfg(ctx, params, sreq.cfg);
+    }
+    if (!decode_batch(ctx, st, tokens.data(), pos.data(), seq.data(), want.data(), n, dev ? &sreq : nullptr, n_audio_ctx)) return false;
+    if (st.dtw_qk_last.size() != (size_t) n * n_audio_ctx * ctx.dtw_heads.size()) { set_error("dtw: the pass returned no alignment weights"); return false; }
+    const int64_t t0 = time_us();
     std::vector<int32_t> ti, tj;
     dtw_path(st.dtw_qk_last.data(), n, n_audio_ctx, (int) ctx.dtw_heads.size(), n_frames / 2, sot_len, 7, ti, tj);
     dtw_assign(ti, tj, seek, vocab.token_eot, st.result_all, i_segment, n_segments);
+    counter_add(10, 1e-3 * (double) (time_us() - t0));           // host DTW ms (wb200_counters)
     return true;
 }
 } // namespace
@@ -1127,7 +1135,6 @@ WB_EXPORT int whisper_full_parallel(struct whisper_context * ctx, struct whisper
 WB_EXPORT int wb200_full_batch_ex(struct whisper_context * ctx, struct whisper_full_params params, const float * const * samples,
                                   const int * n_samples, int n_chunks, struct whisper_state ** states_out, int flags) {
     if (!ctx || !samples || !n_samples || !states_out || n_chunks <= 0) return -1;
-    if (ctx->params.dtw_token_timestamps) { set_error("wb200_full_batch: DTW token timestamps are not available in the lock-step driver"); logf(LOG_ERROR, "%s: %s\n", __func__, last_error()); return -1; }
     if ((flags & 1) && !ctx->replicas.empty()) { set_error("wb200_full_batch: device-pointer input needs a single-GPU context (WB200_DEVICES is set)"); logf(LOG_ERROR, "%s: %s\n", __func__, last_error()); return -1; }
     if (params.vad) { set_error("wb200_full_batch: params.vad is not applied to pre-cut chunks; run whisper_vad_* first"); logf(LOG_ERROR, "%s: %s\n", __func__, last_error()); return -1; }
     int S = ctx->model.dec_tm ? 64 : 8;          // concurrent sequences: one row each in the decode pass (64 rows per launch of the persistent kernel)

@@ -223,7 +223,7 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
     {   // the persistent decode kernel (wb_decode_mk.cu) reads the decoder matrices in the tile-major layout; WB200_MEGAKERNEL=0
         // keeps them planar for the kernel-per-op chain (odd shapes always use the chain; K-quants need whole super-blocks: d % 256)
         const char * e = getenv("WB200_MEGAKERNEL");
-        m.dec_tm = !m.force_planar && (!e || atoi(e) != 0) && wt_tm_rec_bytes(wt) > 0 && d % 128 == 0 && (!wt_is_kquant(wt) || d % 256 == 0) &&
+        m.dec_tm = (!e || atoi(e) != 0) && wt_tm_rec_bytes(wt) > 0 && d % 128 == 0 && (!wt_is_kquant(wt) || d % 256 == 0) &&
                    hp.n_text_head * 64 == d && hp.n_text_state == d;
     }
     if (!alloc_qmat(m, wt, V, d, m.d_te, m.dec_tm)) return false;

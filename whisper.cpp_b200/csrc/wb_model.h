@@ -64,7 +64,6 @@ struct Model {
     int     wtype = WT_F16;          // type of every 2-D weight (src/whisper.cpp:1549-1559)
     int     mtype = 0;               // e_model (1 tiny .. 5 large)
     int     n_loaded = 0;            // 0 => weight-less test stub (src/whisper.cpp:1947-1948)
-    bool    force_planar = false;    // set before loading: keep the decoder weights planar (kernel chain), as DTW contexts need
     int     device = 0;
     bool    dec_tm = false;          // decoder matrices + token embedding are in the tile-major layout (persistent decode kernel)
     int64_t t_load_us = 0;

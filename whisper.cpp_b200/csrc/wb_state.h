@@ -78,8 +78,7 @@ struct whisper_state {
 
     std::unique_ptr<wb::FrontEnd> fe_own;      // PCM + mel of this state (handed back to the context's pool by whisper_free_state)
     wb::FrontEnd & fe;                         // = *fe_own
-    wb::Engine * eng = nullptr;                // own engine (DTW contexts), or the engine shared by all states of the context
-    std::unique_ptr<wb::Engine> own_eng;
+    wb::Engine * eng = nullptr;                // the engine of the context's pool (null for result-only and engine-less test states)
     wb::Group * group = nullptr;               // non-null: this state lives in the context's pool; its encode/decode requests rendezvous
                                                // with those of the other states that are inside whisper_full* at the same time
     bool in_group_call = false;                // between Group::enter and Group::leave
@@ -163,6 +162,7 @@ struct Group {
     Engine eng;
     bool scripted = false;                      // test hook: no engine, decodes leave zero logits
     const Model * model = nullptr;
+    std::vector<std::pair<int, int>> dtw_heads; // alignment heads of the context (DTW token timestamps): the engine's capture table
     // ---- slots: one cross-KV slot + `cps` self-KV cells per state; the pool grows (contents preserved) while no pass is in flight
     int cap = 0, cps = 0;
     std::vector<uint8_t> slot_used;
@@ -184,6 +184,7 @@ struct Group {
         int seek = 0, n_ctx = 0;                // encode
         const int * tokens = nullptr, * pos = nullptr, * seq = nullptr; const int8_t * want = nullptr; int n = 0;   // decode
         const SampReq * samp = nullptr;
+        int dtw_n_ctx = 0;                       // > 0: a DTW pass; capture its alignment-head queries and compute its weights over this many audio positions
         const int * x_cells = nullptr, * x_idx = nullptr, * x_nkv = nullptr; int x_ld = 0;   // explicit self-KV cells / attended lists (relative to the state's range) instead of the KvCells bookkeeping: the ggml-backend plugin passes what the host's KQ_mask says
         bool taken = false;                      // (under mu) some thread took the batch that contains this request
         std::atomic<int> done{0};                // futex word: the member sleeps on its OWN request (no shared mutex to re-acquire on wake-up)
@@ -217,6 +218,6 @@ int64_t time_us();
 bool & tls_pcm_is_device();   // set by the batch driver: the next whisper_pcm_to_mel* `samples` pointer is a device pointer
 // decode one batch through the engine with the reference's KV bookkeeping (whisper_decode_internal, whisper.cpp:2856-2986)
 bool decode_batch(whisper_context & ctx, whisper_state & st, const int * tokens, const int * pos, const int * seq,
-                  const int8_t * want, int n_tokens, const SampReq * samp = nullptr);
+                  const int8_t * want, int n_tokens, const SampReq * samp = nullptr, int dtw_n_ctx = 0);
 bool encode_window(whisper_context & ctx, whisper_state & st, int mel_offset);
 }
