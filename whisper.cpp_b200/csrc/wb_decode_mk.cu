@@ -9,7 +9,8 @@
 // dots like the reference CPU path -- Q8_K super-blocks for Q4_K / Q5_K weights --, f16-rounded Q, f32 softmax); this file changes HOW
 // the ops are scheduled:
 //   * grid = one CTA of 16 warps per SM, launched cooperatively; a phase boundary is a grid barrier instead of a kernel
-//     boundary (the decode step is a chain of ~400 dependent phases of a few microseconds each);
+//     boundary (the decode step is a chain of ~400 dependent phases of a few microseconds each); a pass of 32 rows or more is cut into
+//     partitions (row groups x CTA ranges, MkView) that walk the layers on their own barriers and take turns streaming cross K/V;
 //   * rows handed from one phase to the next are quantised once by their producer ("actq" rows in global memory): a
 //     distributed LayerNorm -> Q8_0 phase, attention epilogues, and a quantise phase after FC1;
 //   * a GEMV phase is cut by row group first: a CTA stages the 16 rows of its group with TMA bulk copies and walks 16-row
@@ -59,47 +60,78 @@ __device__ __forceinline__ void l2_prefetch(const void * p, uint32_t bytes) {
     if (bytes >= 16) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(p), "r"(bytes & ~15u) : "memory");
 }
 
-// Grid barrier.  Arrival = one atomic on a counter; the LAST CTA to arrive releases everybody by writing one flag per CTA
-// (each on its own 128-byte line), and every other CTA polls only its own flag.
-__device__ __noinline__ void mk_grid_sync(const MkArgs & a, unsigned long long target) {
+// What a phase function knows about who shares the phase with its CTA: the CTA's index among the `nc` CTAs of its partition and the
+// partition's rows [row0, row0 + n_tok).  part = -1: the whole grid (logits).
+struct MkView { int ci, nc, row0, n_tok, part; };
+
+// words of MkArgs::bar: [0] arrival counter of the grid, [8] error flag, [16 + 16*cta + w] release flags of a CTA (one 128-byte line per CTA;
+// w = 0: grid barrier, 1 + p: barrier of partition p -- a flag only ever sees the targets of one counter, so it stays monotonic when the
+// number of partitions changes from pass to pass), then one line per partition counter and one for the turn word
+__device__ __forceinline__ unsigned long long * mk_bar_tail(const MkArgs & a, int i) { return a.bar + 16 + 16 * (size_t) gridDim.x + 16 * i; }
+constexpr int MK_TRACE_TURN = 2100;     // trace slot: SM clocks partition 0 waited for its turn to stream (accumulates)
+
+// Barrier of the CTAs of a view.  Arrival = one atomic on the view's counter; the LAST CTA to arrive releases the others by writing one
+// flag per CTA (each on its own 128-byte line), and every other CTA polls only its own flag.
+// turn = 1 (the barrier in front of the cross-attention, several partitions): the releasing CTA first waits until fewer than
+// a.turn_slots partitions are streaming K/V and takes a slot; turn = 2 (the barrier behind it): the partition gives the slot back.  A
+// partition that holds a slot never waits for another partition, and all CTAs are resident: the wait always ends.
+__device__ __noinline__ void mk_grid_sync(const MkArgs & a, const MkView v, unsigned long long target, int turn) {
+    unsigned long long * const cnt = v.part < 0 ? a.bar : mk_bar_tail(a, v.part);
+    unsigned long long * const turn_w = mk_bar_tail(a, MK_MAX_PARTS);
+    if (a.n_part == 1) turn = 0;
     __syncthreads();
-    if (a.prefetch & 32) {
+    if ((a.prefetch & 32) && turn != 1) {
         // variant: arrival = a reduction without a return value, and EVERY CTA polls the counter itself -- no dependent chain
         // "atomic returns -> last arriver writes the flags -> the flags become visible" (one L2 round trip less per barrier)
         if (threadIdx.x == 0) {
             __threadfence();
-            asm volatile("red.release.gpu.global.add.u64 [%0], 1;" :: "l"(a.bar) : "memory");
+            asm volatile("red.release.gpu.global.add.u64 [%0], 1;" :: "l"(cnt) : "memory");
             const long long t0 = clock64();
-            unsigned long long v;
+            unsigned long long c;
             for (;;) {
-                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(a.bar) : "memory");
-                if (v >= target) break;
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(c) : "l"(cnt) : "memory");
+                if (c >= target) break;
                 if (clock64() - t0 > (6LL << 30)) { *a.err = 1; __threadfence_system(); __trap(); }
             }
+            if (turn == 2 && v.ci == 0) atomicAdd(turn_w, ~0ULL);
         }
         __syncthreads();
         return;
     }
     if (threadIdx.x == 0) {
         __threadfence();
-        const unsigned long long old = atomicAdd(a.bar, 1ULL);
+        const unsigned long long old = atomicAdd(cnt, 1ULL);
         SM_FLAG[2] = (old + 1 == target);
-        if (old + 1 == target) __threadfence();                  // the last arriver acquires what the others released
+        if (old + 1 == target) {
+            __threadfence();                                     // the last arriver acquires what the others released
+            if (turn == 1) {
+                const long long t0 = clock64();
+                for (;;) {
+                    unsigned long long s;
+                    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(s) : "l"(turn_w) : "memory");
+                    if (s < (unsigned long long) a.turn_slots && atomicCAS(turn_w, s, s + 1) == s) break;
+                    if (clock64() - t0 > (6LL << 30)) { *a.err = 1; __threadfence_system(); __trap(); }
+                }
+                if (a.trace && v.part == 0) atomicAdd(reinterpret_cast<unsigned long long *>(a.trace) + MK_TRACE_TURN, (unsigned long long) (clock64() - t0));
+            }
+        }
     }
     __syncthreads();
+    unsigned long long * const flags = a.bar + 16 + 16 * (size_t) (blockIdx.x - v.ci) + (v.part + 1);
     if (SM_FLAG[2]) {
-        for (int i = threadIdx.x; i < (int) gridDim.x; i += MK_THREADS)
-            asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(a.bar + 16 + 16 * i), "l"(target) : "memory");
+        for (int i = threadIdx.x; i < v.nc; i += MK_THREADS)
+            asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(flags + 16 * i), "l"(target) : "memory");
     } else if (threadIdx.x == 0) {
-        const unsigned long long * f = a.bar + 16 + 16 * blockIdx.x;
+        const unsigned long long * f = flags + 16 * v.ci;
         const long long t0 = clock64();
-        unsigned long long v;
+        unsigned long long c;
         for (;;) {
-            asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(f) : "memory");
-            if (v >= target) break;
+            asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(c) : "l"(f) : "memory");
+            if (c >= target) break;
             if (clock64() - t0 > (6LL << 30)) { *a.err = 1; __threadfence_system(); __trap(); }    // ~3 s: a CTA never arrived
         }
     }
+    if (turn == 2 && v.ci == 0 && threadIdx.x == 0) atomicAdd(turn_w, ~0ULL);
     __syncthreads();
 }
 
@@ -152,11 +184,11 @@ __device__ __forceinline__ void mk_store_q(uint8_t * dst, int K, int t, int e0, 
 }
 
 // LayerNorm (ggml-cpu/ops.cpp:3698-3765, two passes, then mul/add whisper.cpp:2536-2543) of the f32 residual rows, quantised into
-// `dst`.  Distributed: CTA r normalises row r (one warp per 128 values); followed by a grid barrier.
+// `dst`.  Distributed: CTA r of the view normalises its row r (one warp per 128 values); followed by a barrier.
 template <int WT>
-__device__ __noinline__ void mk_lnq(const MkArgs & a, const float * src, int K, const float * __restrict__ ln_w, const float * __restrict__ ln_b, uint8_t * dst) {
+__device__ __noinline__ void mk_lnq(const MkArgs & a, const MkView v, const float * src, int K, const float * __restrict__ ln_w, const float * __restrict__ ln_b, uint8_t * dst) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int row = blockIdx.x; row < a.n_tok; row += gridDim.x) {
+    for (int row = v.row0 + v.ci; row < v.row0 + v.n_tok; row += v.nc) {
         const bool act = warp < (K >> 7);
         const int e0 = warp * 128 + lane * 4;
         float4 v = act ? __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0)) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -226,12 +258,12 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const float * src, int K, 
 
 // quantise f32 rows (no LayerNorm) into the actq format: one warp per (row, 128 values); followed by a grid barrier
 template <int WT>
-__device__ __noinline__ void mk_q8_rows(const MkArgs & a, const float * src, int K, uint8_t * dst) {
-    const int lane = threadIdx.x & 31, wg = blockIdx.x * MK_WARPS + (threadIdx.x >> 5), nwg = gridDim.x * MK_WARPS;
+__device__ __noinline__ void mk_q8_rows(const MkView v, const float * src, int K, uint8_t * dst) {
+    const int lane = threadIdx.x & 31, wg = v.ci * MK_WARPS + (threadIdx.x >> 5), nwg = v.nc * MK_WARPS;
     const int cpr = K >> 7;
-    int row = wg / cpr, ch = wg - row * cpr;
+    int row = v.row0 + wg / cpr, ch = wg - (wg / cpr) * cpr;
     const int drow = nwg / cpr, dch = nwg - drow * cpr;
-    for (; row < a.n_tok; ) {
+    for (; row < v.row0 + v.n_tok; ) {
         const int e0 = ch * 128 + lane * 4;
         const float4 y = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0));
         if (WT == WT_F16) {
@@ -252,13 +284,13 @@ __device__ __noinline__ void mk_q8_rows(const MkArgs & a, const float * src, int
     }
 }
 
-// K-quants: f32 rows -> Q8_K rows, one warp per (row, super-block); followed by a grid barrier
-__device__ __noinline__ void mk_q8k_rows(const MkArgs & a, const float * src, int K, uint8_t * dst) {
-    const int lane = threadIdx.x & 31, nsb = K >> 8, n = a.n_tok * nsb;
-    for (int p = blockIdx.x * MK_WARPS + (threadIdx.x >> 5); p < n; p += gridDim.x * MK_WARPS) {
-        const int row = p / nsb, e0 = (p - row * nsb) * 256 + lane * 4;
-        const float4 y0 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0));
-        const float4 y1 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0 + 128));
+// K-quants: f32 rows (`lds` floats apart) -> Q8_K rows, one warp per (row, super-block); followed by a barrier
+__device__ __noinline__ void mk_q8k_rows(const MkView v, const float * src, int lds, int K, uint8_t * dst) {
+    const int lane = threadIdx.x & 31, nsb = K >> 8, n = v.n_tok * nsb;
+    for (int p = v.ci * MK_WARPS + (threadIdx.x >> 5); p < n; p += v.nc * MK_WARPS) {
+        const int row = v.row0 + p / nsb, e0 = (p - (row - v.row0) * nsb) * 256 + lane * 4;
+        const float4 y0 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * lds + e0));
+        const float4 y1 = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * lds + e0 + 128));
         float amax = fabsf(y0.x), mx = y0.x;
         q8k_pick(amax, mx, fabsf(y0.y), y0.y); q8k_pick(amax, mx, fabsf(y0.z), y0.z); q8k_pick(amax, mx, fabsf(y0.w), y0.w);
         q8k_pick(amax, mx, fabsf(y1.x), y1.x); q8k_pick(amax, mx, fabsf(y1.y), y1.y); q8k_pick(amax, mx, fabsf(y1.z), y1.z); q8k_pick(amax, mx, fabsf(y1.w), y1.w);
@@ -287,12 +319,12 @@ struct MkEpi {
     uint8_t * qout = nullptr;            // PAIR epilogue: quantised rows [64][N] (+ block scales) for the next GEMV
 };
 
-// L2 prefetch of weight tiles for a later GEMV phase (tile-major: the records of a tile are contiguous); every tile once per grid
-__device__ __noinline__ void mk_prefetch_w(const QMat & W) {
+// L2 prefetch of weight tiles for a later GEMV phase (tile-major: the records of a tile are contiguous); every tile once per view
+__device__ __noinline__ void mk_prefetch_w(const MkView v, const QMat & W) {
     if (threadIdx.x != MK_THREADS - 32) return;
     const int n_tiles = (W.N + 15) >> 4;
     const uint32_t tile_bytes = (uint32_t) (W.K / wt_tm_rec_k(W.type)) * wt_tm_rec_bytes(W.type);
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
+    for (int tile = v.ci; tile < n_tiles; tile += v.nc)
         l2_prefetch(reinterpret_cast<const uint8_t *>(W.base) + (size_t) tile * tile_bytes, tile_bytes);
 }
 
@@ -451,7 +483,7 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 // PAIR (FC1): tiles are dealt out in pairs = 32 consecutive output features, and the epilogue writes GELU(y) straight into the
 // quantised-row format FC2 consumes (one warp = one Q8_0 block of one row) -- no f32 round trip, no extra phase.
 template <int WT, bool PAIR>
-__device__ __noinline__ void mk_gemv(const MkArgs & a, const QMat & W, const uint8_t * x, const MkEpi & e, int fb = -1) {
+__device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, const MkEpi & e, int fb = -1) {
     constexpr int REC = (WT == WT_Q4_0) ? 288 : (WT == WT_Q5_0 ? 352 : (WT == WT_Q8_0 ? 544 : 512));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;             // bytes of the qs part of a record
     constexpr int RK = (WT == WT_F16) ? 16 : 32;                 // K values per record
@@ -464,9 +496,9 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const QMat & W, const uin
     const int n_tiles = (N + 15) >> 4, nrec = K / RK, nb = K >> 5;
     const int rowb = (WT == WT_F16) ? K * 2 : K, SW = (rowb >> 2) + 4;
     const int RG = (16 * (rowb + 16) <= MK_MAXTOK * (MK_ROWB + 16)) ? 16 : 8;   // rows per CTA (what fits the staging area)
-    const int NGc = (a.n_tok + RG - 1) / RG;
-    const int grp = blockIdx.x % NGc, ci = blockIdx.x / NGc, cg = ((int) gridDim.x - grp + NGc - 1) / NGc;   // row group, index / count of its CTAs
-    const int t_base = grp * RG, nt = min(RG, a.n_tok - t_base), NH = (nt + 7) >> 3;
+    const int NGc = (v.n_tok + RG - 1) / RG;
+    const int grp = v.ci % NGc, ci = v.ci / NGc, cg = (v.nc - grp + NGc - 1) / NGc;   // row group, index / count of its CTAs
+    const int t_base = v.row0 + grp * RG, nt = min(RG, v.n_tok - grp * RG), NH = (nt + 7) >> 3;
     const int n_units = n_tiles / TU;                            // PAIR: N is a multiple of 32
     const int upc = ci < n_units ? (n_units - ci + cg - 1) / cg : 0;            // units of this CTA: ci, ci + cg, ...
     const int n_it = (upc * TU + TP - 1) / TP, upi = n_it ? (upc + n_it - 1) / n_it : 0;   // iterations, units per iteration (even split)
@@ -566,7 +598,7 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const QMat & W, const uin
 // 45.6 MB stream).  A lane requests 8 records of its tile at once; the rows of the CTA's group are staged as in mk_gemv.  A row's result
 // is one accumulator over the blocks in ascending order: independent of the batch.
 template <int WT>
-__device__ __noinline__ void mk_logits_warp(const MkArgs & a, const QMat & W, const uint8_t * x, float * out) {
+__device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, float * out) {
     constexpr bool KQ = mk_kq(WT);
     constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 : 512));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
@@ -577,9 +609,9 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const QMat & W, co
     const int n_tiles = (N + 15) >> 4, nrec = K / RK, nb = K >> 5;
     const int rowb = (WT == WT_F16) ? K * 2 : K, SW = (rowb >> 2) + 4;
     const int RG = (16 * (rowb + 16) <= MK_MAXTOK * (MK_ROWB + 16)) ? 16 : 8;
-    const int NGc = (a.n_tok + RG - 1) / RG;
-    const int grp = blockIdx.x % NGc, ci = blockIdx.x / NGc, cg = ((int) gridDim.x - grp + NGc - 1) / NGc;
-    const int t_base = grp * RG, nt = min(RG, a.n_tok - t_base), NH = (nt + 7) >> 3;
+    const int NGc = (v.n_tok + RG - 1) / RG;
+    const int grp = v.ci % NGc, ci = v.ci / NGc, cg = (v.nc - grp + NGc - 1) / NGc;
+    const int t_base = v.row0 + grp * RG, nt = min(RG, v.n_tok - grp * RG), NH = (nt + 7) >> 3;
     uint32_t stage_parity;
     {
         const int ph = SM_FLAG[4];
@@ -802,13 +834,13 @@ __device__ __forceinline__ float attn_merge(const float * pp, int nw, int dim, f
 // with 64 rows x 20 heads every item has its warps in the first round).  A lane owns a key quarter; the cells and the K / V pieces of
 // four key groups are requested together, so a row with 200 keys costs a handful of memory round trips instead of one per group.
 template <int WT>
-__device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkLayer & L) {
+__device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkView v, const MkLayer & L) {
     constexpr int WPI = 2, SB = 2, CV = 16;                      // warps per item, key groups in flight together (double-buffered), cell indices per lane requested at once
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, grp = warp / WPI, hw = warp % WPI;
-    const int d = a.d, H = a.n_head, n_pairs = a.n_tok * H;
+    const int d = a.d, H = a.n_head, n_pairs = v.n_tok * H;
     const int kslot = lane >> 2, r = lane & 3;
-    for (int p = blockIdx.x * (MK_WARPS / WPI) + grp; p < n_pairs; p += gridDim.x * (MK_WARPS / WPI)) {
-        const int t = p / H, h = p - t * H;
+    for (int p = v.ci * (MK_WARPS / WPI) + grp; p < n_pairs; p += v.nc * (MK_WARPS / WPI)) {
+        const int t = v.row0 + p / H, h = p - (t - v.row0) * H;
         const int nk = a.nkv[t];
         const int * cells = a.idx + (size_t) t * a.ld_idx;
         float q[16];
@@ -864,7 +896,7 @@ __device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkLayer & L) {
 // cross-attention over the n_keys padded encoder positions, zero rows included (whisper.cpp:2688-2705).
 // K and V of a window live HEAD-MAJOR in HBM ([layer][head][key][64], written that way by the cross GEMM's epilogue): the keys of one
 // (row, head) pair are one contiguous 192 KB stream instead of 128-byte pieces 2.5 KB apart.
-// Work unit = one (row, head) pair over ALL keys; CTA b takes the contiguous range of pairs [b*P/G, (b+1)*P/G).  Warp w, key slot s owns
+// Work unit = one (row, head) pair over ALL keys; CTA b of the view takes the contiguous range [b*P/G, (b+1)*P/G) of its P pairs.  Warp w, key slot s owns
 // key 8w+s of every 128-key chunk; chunks are copied three ahead with cp.async into a 4-deep ring in shared memory (the GEMV staging
 // area, idle here); every thread reads back only the 64 bytes it copied itself, so the ring needs no barrier -- it is an asynchronous
 // extension of the register file (96 KB in flight per SM; a 6-deep ring was measured slower: the 40 KB of L1 it takes away cost the other
@@ -878,12 +910,12 @@ static_assert(MK_OFF_QSM + 2 * 64 * 4 <= MK_OFF_PART, "the cp.async ring must fi
 __device__ __forceinline__ void cp_wait_ring() { asm volatile("cp.async.wait_group %0;" :: "n"(MK_RING - 1) : "memory"); }
 
 template <int WT>
-__device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) {
+__device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, const MkLayer & L) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int d = a.d, H = a.n_head, nchp = a.n_keys / MK_XKEYS;               // chunks per pair
-    const unsigned P = (unsigned) (a.n_tok * H), G = min(gridDim.x, P);
-    if (blockIdx.x >= G) return;
-    const unsigned p0 = (blockIdx.x * P) / G, p1 = ((blockIdx.x + 1) * P) / G;
+    const unsigned P = (unsigned) (v.n_tok * H), G = min((unsigned) v.nc, P), P0 = (unsigned) (v.row0 * H);   // pairs of the view: P0 .. P0 + P - 1
+    if ((unsigned) v.ci >= G) return;
+    const unsigned p0 = P0 + ((unsigned) v.ci * P) / G, p1 = P0 + (((unsigned) v.ci + 1) * P) / G;
     // loader state: chunk being fetched
     unsigned pl = p0, il = 0;
     int jl = 0, tl_ = (int) p0 / H, hl = (int) p0 - tl_ * H;
@@ -957,7 +989,9 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) 
             const int dim = warp * 32 + lane;
             float M, Lsum;
             const float o = attn_merge(SM_PART + buf * MK_WARPS * MK_PART, MK_WARPS, dim, M, Lsum);
-            mk_store_q<WT>(mk_kq(WT) ? reinterpret_cast<uint8_t *>(a.qkv) : a.actq, d, t, h * 64 + warp * 32, lane, __fdividef(o, Lsum));
+            // K-quants: the f32 row goes where the Q of row t was (a.qkv, rows 3d apart): whatever phase the other partitions are in, they
+            // touch their own rows only
+            mk_store_q<WT>(mk_kq(WT) ? reinterpret_cast<uint8_t *>(a.qkv) : a.actq, mk_kq(WT) ? 3 * d : d, t, h * 64 + warp * 32, lane, __fdividef(o, Lsum));
         }
         buf ^= 1;
         lane_init(A);
@@ -968,90 +1002,97 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkLayer & L) 
 }
 
 // DTW: copy the alignment-head slices of the cross-Q rows (complete after the barrier that ended phase 6) into the capture buffer
-__device__ __noinline__ void mk_dtw_capture(const MkArgs & a, const MkLayer & L) {
-    dtw_capture_rows(a.q2, a.d, a.cap_row, a.n_tok, L.cap_mask, L.cap_head0, a.cap, a.cap_rows, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
+__device__ __noinline__ void mk_dtw_capture(const MkArgs & a, const MkView v, const MkLayer & L) {
+    dtw_capture_rows(a.q2 + (size_t) v.row0 * a.d, a.d, a.cap_row + v.row0, v.n_tok, L.cap_mask, L.cap_head0, a.cap, a.cap_rows, v.ci * blockDim.x + threadIdx.x, v.nc * blockDim.x);
 }
 
-#define MK_SYNC() do { MK_STAMP(); target += gridDim.x; mk_grid_sync(a, target); MK_STAMP(); } while (0)
-#define MK_SYNC_Q() do { target += gridDim.x; mk_grid_sync(a, target); } while (0)      // without trace stamps (24 per layer for every format)
+#define MK_SYNC_T(turn) do { MK_STAMP(); target += v.nc; mk_grid_sync(a, v, target, turn); MK_STAMP(); } while (0)
+#define MK_SYNC() MK_SYNC_T(0)
+#define MK_SYNC_Q(turn) do { target += v.nc; mk_grid_sync(a, v, target, turn); } while (0)   // without trace stamps (24 per layer for every format)
 
 template <int WT, bool TRACE>
 __global__ void __launch_bounds__(MK_THREADS, 1)
 k_decode_pass(const __grid_constant__ MkArgs a) {
     if (threadIdx.x == 0) { mbar_init(SM_MBAR, 1); SM_FLAG[4] = 0; mbar_fence_init(); }
     __syncthreads();
-    unsigned long long target = a.bar_base;
+    // this CTA's partition: the view every phase of the layer loop works in
+    int part = 0;
+    while (part + 1 < a.n_part && (int) blockIdx.x >= mk_partition(part + 1, a.n_part, gridDim.x, a.n_tok).c0) ++part;
+    const MkPart pt = mk_partition(part, a.n_part, gridDim.x, a.n_tok);
+    const MkView v = { (int) blockIdx.x - pt.c0, pt.nc, pt.row0, pt.n_tok, part };
+    const MkView vg = { (int) blockIdx.x, (int) gridDim.x, 0, a.n_tok, -1 };      // the whole grid: the partitions join for the logits
+    unsigned long long target = a.part_base[part];
     int n_stamp = 0;
     const int d = a.d;
     const bool pf_w = a.prefetch & 1;
     MK_STAMP();
-    if (pf_w) mk_prefetch_w(a.layers[0].qkv);
+    if (pf_w) mk_prefetch_w(v, a.layers[0].qkv);
 
     for (int l = 0; l < a.n_layer; ++l) {
         const MkLayer & L = a.layers[l];
         MkEpi e;
         // 1: LN -> quantised rows (whisper.cpp:2536-2543)
-        mk_lnq<WT>(a, a.x, d, L.ln0_w, L.ln0_b, a.actq);
-        if (pf_w) mk_prefetch_w(L.o);
+        mk_lnq<WT>(a, v, a.x, d, L.ln0_w, L.ln0_b, a.actq);
+        if (pf_w) mk_prefetch_w(v, L.o);
         MK_SYNC();
         // 2: QKV + KV append (2545-2599)
         e = MkEpi(); e.bias = L.qkv_bias; e.scale = L.qkv_scale; e.out = a.qkv; e.kc = L.kc; e.vc = L.vc; e.kv_d = d;
-        mk_gemv<WT, false>(a, L.qkv, a.actq, e, (TRACE && l == 1) ? 2048 + 0 : -1);
+        mk_gemv<WT, false>(a, v, L.qkv, a.actq, e, (TRACE && l == 1) ? 2048 + 0 : -1);
         MK_SYNC();
         // 3: self-attention (2603-2625) -> quantised rows for the O projection
-        if (pf_w) mk_prefetch_w(L.cq);
-        mk_attn_self<WT>(a, L);
-        if (mk_kq(WT)) { MK_SYNC_Q(); mk_q8k_rows(a, a.q2, d, a.actq); }     // K-quants: f32 rows -> Q8_K (timed with the attention)
+        if (pf_w) mk_prefetch_w(v, L.cq);
+        mk_attn_self<WT>(a, v, L);
+        if (mk_kq(WT)) { MK_SYNC_Q(0); mk_q8k_rows(v, a.q2, d, d, a.actq); }     // K-quants: f32 rows -> Q8_K (timed with the attention)
         MK_SYNC();
         // 4: O + residual (2647-2659)
-        if (pf_w) mk_prefetch_w(L.co);
+        if (pf_w) mk_prefetch_w(v, L.co);
         e = MkEpi(); e.bias = L.o_bias; e.res = a.x; e.out = a.x;
-        mk_gemv<WT, false>(a, L.o, a.actq, e, (TRACE && l == 1) ? 2048 + 8 : -1);
+        mk_gemv<WT, false>(a, v, L.o, a.actq, e, (TRACE && l == 1) ? 2048 + 8 : -1);
         MK_SYNC();
         // 5: LN -> quantised rows
-        mk_lnq<WT>(a, a.x, d, L.lnc_w, L.lnc_b, a.actq);
-        if (pf_w) mk_prefetch_w(L.fc1);
+        mk_lnq<WT>(a, v, a.x, d, L.lnc_w, L.lnc_b, a.actq);
+        if (pf_w) mk_prefetch_w(v, L.fc1);
         MK_SYNC();
         // 6: cross Q (2661-2681)
         e = MkEpi(); e.bias = L.cq_bias; e.out = a.q2;
-        mk_gemv<WT, false>(a, L.cq, a.actq, e, (TRACE && l == 1) ? 2048 + 16 : -1);
-        MK_SYNC();
+        mk_gemv<WT, false>(a, v, L.cq, a.actq, e, (TRACE && l == 1) ? 2048 + 16 : -1);
+        MK_SYNC_T(1);                                            // the partition takes its turn to stream K/V ...
         // 7: cross-attention (2688-2705); DTW passes first keep the alignment-head queries of their flagged rows
-        if (pf_w) mk_prefetch_w(L.fc2);
-        if (a.cap != nullptr && L.cap_mask != 0u) mk_dtw_capture(a, L);
-        mk_attn_cross<WT>(a, L);
-        if (mk_kq(WT)) { MK_SYNC_Q(); mk_q8k_rows(a, a.qkv, d, a.actq); }
-        MK_SYNC();
+        if (pf_w) mk_prefetch_w(v, L.fc2);
+        if (a.cap != nullptr && L.cap_mask != 0u) mk_dtw_capture(a, v, L);
+        mk_attn_cross<WT>(a, v, L);
+        if (mk_kq(WT)) { MK_SYNC_Q(2); mk_q8k_rows(v, a.qkv, 3 * d, d, a.actq); }   // ... and gives it back at the first barrier behind the stream
+        MK_SYNC_T(mk_kq(WT) ? 0 : 2);
         // 8: cross O + residual (2754-2766)
         e = MkEpi(); e.bias = L.co_bias; e.res = a.x; e.out = a.x;
-        mk_gemv<WT, false>(a, L.co, a.actq, e, (TRACE && l == 1) ? 2048 + 24 : -1);
+        mk_gemv<WT, false>(a, v, L.co, a.actq, e, (TRACE && l == 1) ? 2048 + 24 : -1);
         MK_SYNC();
         // 9: LN -> quantised rows
-        mk_lnq<WT>(a, a.x, d, L.lnm_w, L.lnm_b, a.actq);
-        if (pf_w) { if (l + 1 < a.n_layer) mk_prefetch_w(a.layers[l + 1].qkv); else if (a.want_logits) mk_prefetch_w(a.te); }
+        mk_lnq<WT>(a, v, a.x, d, L.lnm_w, L.lnm_b, a.actq);
+        if (pf_w) { if (l + 1 < a.n_layer) mk_prefetch_w(v, a.layers[l + 1].qkv); else if (a.want_logits) mk_prefetch_w(vg, a.te); }
         MK_SYNC();
         // 10: FC1 + GELU (2770-2794), then the rows are quantised for FC2
         if (mk_kq(WT)) {                                         // K-quants: f32 GELU rows, then a Q8_K phase (trace slot "10b h->q8")
             e = MkEpi(); e.bias = L.fc1_bias; e.act = 1; e.out = a.h;
-            mk_gemv<WT, false>(a, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
-            MK_STAMP(); MK_SYNC_Q(); MK_STAMP();
-            mk_q8k_rows(a, a.h, 4 * d, a.hq);
+            mk_gemv<WT, false>(a, v, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
+            MK_STAMP(); MK_SYNC_Q(0); MK_STAMP();
+            mk_q8k_rows(v, a.h, 4 * d, 4 * d, a.hq);
         } else {
             e = MkEpi(); e.bias = L.fc1_bias; e.act = 1; e.qout = a.hq;
-            mk_gemv<WT, true>(a, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
+            mk_gemv<WT, true>(a, v, L.fc1, a.actq, e, (TRACE && l == 1) ? 2048 + 32 : -1);
             MK_STAMP(); MK_STAMP();                              // (trace slot of the former FC1 -> Q8_0 phase)
         }
         MK_SYNC();
         // 11: FC2 + residual (2797-2806)
         e = MkEpi(); e.bias = L.fc2_bias; e.res = a.x; e.out = a.x;
-        mk_gemv<WT, false>(a, L.fc2, a.hq, e, (TRACE && l == 1) ? 2048 + 40 : -1);
+        mk_gemv<WT, false>(a, v, L.fc2, a.hq, e, (TRACE && l == 1) ? 2048 + 40 : -1);
         MK_SYNC();
     }
     if (a.want_logits) {                                         // final LN + logits (2811-2827)
-        mk_lnq<WT>(a, a.x, d, a.lnf_w, a.lnf_b, a.actq);
-        MK_SYNC();
-        if (a.prefetch & 16) mk_logits_warp<WT>(a, a.te, a.actq, a.logits);
-        else { MkEpi e; e.out = a.logits; mk_gemv<WT, false>(a, a.te, a.actq, e); }
+        mk_lnq<WT>(a, v, a.x, d, a.lnf_w, a.lnf_b, a.actq);
+        MK_STAMP(); mk_grid_sync(a, vg, a.bar_base + gridDim.x, 0); MK_STAMP();
+        if (a.prefetch & 16) mk_logits_warp<WT>(a, vg, a.te, a.actq, a.logits);
+        else { MkEpi e; e.out = a.logits; mk_gemv<WT, false>(a, vg, a.te, a.actq, e); }
         MK_STAMP();
     }
 }
@@ -1059,7 +1100,8 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
 bool mk_cross_head_major() {
     return true;
 }
-int mk_barriers(int wtype, int n_layer, bool want_logits) { return (wt_is_kquant(wtype) ? 14 : 11) * n_layer + (want_logits ? 1 : 0); }
+int mk_layer_barriers(int wtype) { return wt_is_kquant(wtype) ? 14 : 11; }
+size_t mk_bar_words(int n_sm) { return 16 + 16 * (size_t) n_sm + 16 * (MK_MAX_PARTS + 1); }
 bool mk_supported(int wtype) { return wtype == WT_F16 || wt_is_block32(wtype) || wt_is_kquant(wtype); }
 size_t mk_smem_bytes(int, int) { return MK_SMEM; }
 int mk_max_rows() { return MK_MAXTOK; }

@@ -18,6 +18,18 @@ struct MkLayer {                      // one text layer: weights (model) + this 
     uint32_t cap_mask; int cap_head0; // DTW: alignment heads of this layer (bit h = head h) and the capture head of the lowest (wb_dtw_kernel.cuh)
 };
 
+// A pass with enough rows is cut into partitions: partition p owns whole 16-row groups [p*G/NP, (p+1)*G/NP) of the G row groups and the
+// CTAs [p*n_cta/NP, (p+1)*n_cta/NP), and walks the layers on its own barrier, so that one partition streams cross K/V from HBM while
+// the others are in their latency-bound phases.  A row's arithmetic does not depend on how many CTAs share a phase: NP changes no bit.
+constexpr int MK_MAX_PARTS = 4;
+struct MkPart { int c0, nc, row0, n_tok; };                       // first CTA / CTAs, first row / rows of a partition
+__host__ __device__ inline MkPart mk_partition(int p, int n_part, int n_cta, int n_tok) {
+    const int G = (n_tok + 15) >> 4, g0 = p * G / n_part, g1 = (p + 1) * G / n_part;
+    const int c0 = p * n_cta / n_part, c1 = (p + 1) * n_cta / n_part;
+    const int r0 = g0 * 16, r1 = g1 * 16 < n_tok ? g1 * 16 : n_tok;
+    return MkPart{ c0, c1 - c0, r0, r1 - r0 };
+}
+
 struct MkArgs {
     const MkLayer * layers; int n_layer;
     int d, n_head, n_tok, n_keys, ld_idx, n_vocab, want_logits;
@@ -30,32 +42,26 @@ struct MkArgs {
     float * h;                        // FC1 + GELU output [R][4d]
     uint8_t * actq, * hq;             // quantised rows handed between phases: K = d (>= R*d*2 + R*d/8 bytes) and K = 4d
     float * xpart; int * xcnt;        // cross-attention partials [R*H][16][66] and arrival counters [R*H]
-    unsigned long long * bar;         // grid barrier: [0] arrival counter (monotonic, never reset), [16 + 16*cta] release flag of each CTA
-    unsigned long long bar_base;      // its value when this launch starts
+    unsigned long long * bar;         // barriers (mk_bar_words): arrival counters (monotonic, never reset) of the grid and of each partition, release flags per CTA, the turn word
+    unsigned long long bar_base;      // value of the grid counter when this launch starts
+    unsigned long long part_base[MK_MAX_PARTS];   // ... and of the partitions' counters
+    int n_part = 1;                   // partitions of this pass (mk_partition): CTA ranges that walk the layers on their own barriers
+    int turn_slots = 1;               // partitions that may stream cross K/V at the same time
     int * err;                        // set to 1 when a barrier wait times out
     long long * trace;                // optional: phase time stamps of CTA 0 (see MK_STAMP)
-    float * cap = nullptr; const int * cap_row = nullptr; int cap_rows = 0;   // DTW capture (generation 1 only): null when no row of the pass has a capture index
+    float * cap = nullptr; const int * cap_row = nullptr; int cap_rows = 0;   // DTW capture: null when no row of the pass has a capture index
     int prefetch;                     // bit0: next-phase weights -> L2, bit1: cross KV -> L2 one phase ahead
-    // second generation (wb_decode_mk2.cu) only:
-    int global_sync = 0;              // a row attends to self-KV cells another row GROUP writes in this pass: all groups meet after the KV append
-    int stagger_clk = 0;              // SM cycles between the starts of consecutive row groups
 };
 
-// number of grid barriers one launch passes (host keeps bar_base in step)
-int  mk_barriers(int wtype, int n_layer, bool want_logits);
+// barriers one launch passes: per layer on the partitions' counters (every CTA of partition p arrives at counter p), plus the grid-wide
+// one in front of the logits.  The host keeps bar_base / part_base in step.
+int  mk_layer_barriers(int wtype);
+size_t mk_bar_words(int n_sm);      // 64-bit words of MkArgs::bar
 bool mk_supported(int wtype);
 size_t mk_smem_bytes(int wtype, int d);
 bool mk_cross_head_major();        // cross K/V of a window is expected head-major ([layer][head][key][64])
 int  mk_max_rows();                 // rows (sequences x tokens) one launch can take
 // cooperative launch on `st`; grid = number of SMs.  Returns false (with the error set) when the launch is refused.
 bool mk_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st);
-
-// ---- second generation (wb_decode_mk2.cu): row groups of 16 walk the layers independently, two CTAs per SM ----
-int  mk2_ctas_per_sm();
-bool mk2_supported(int wtype, int d);
-size_t mk2_smem_bytes();
-size_t mk2_bar_words(int n_sm);     // 64-bit words of MkArgs::bar: [0..127] counters (zeroed by mk2_launch), then 16 per CTA (release flags)
-// cooperative launch on `st`; grid = 2 x number of SMs.  a.bar_base must grow by 4096 per launch.
-bool mk2_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st);
 
 } // namespace wb

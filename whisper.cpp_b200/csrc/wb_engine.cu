@@ -67,14 +67,12 @@ bool Engine::init(const Model * model, int cap_windows) {
             set_error("decode: the persistent kernel cannot run on this device/model; set WB200_MEGAKERNEL=0"); return false;
         }
         if (const char * pf = getenv("WB200_MK_PREFETCH")) mk_prefetch = atoi(pf);
-        // WB200_MK_GEN=2 selects the experimental second generation (row groups walking the layers independently, two CTAs per SM):
         // slower than the first generation where it was measured (DESIGN.md section 4), kept for the A/B
-        mk_gen = 1;
-        if (const char * ge = getenv("WB200_MK_GEN")) mk_gen = atoi(ge) == 2 ? 2 : 1;
-        if (use_mk && mk_gen == 2 && !mk2_supported(m->wtype == WT_F32 ? WT_F16 : m->wtype, hp.n_text_state)) mk_gen = 1;
-        mk_stagger_clk = 0;                                       // optional start stagger of the row groups (the cross-attention turns keep them apart)
-        if (const char * sg = getenv("WB200_MK_STAGGER")) mk_stagger_clk = atoi(sg);
-        if (use_mk && !mk_bar.alloc(std::max<size_t>(32 + 16 * (size_t) n_sm, mk2_bar_words(n_sm)), true)) return false;
+        if (use_mk && !mk_bar.alloc(mk_bar_words(n_sm), true)) return false;
+        // WB200_MK_PARTS=1..4: partitions of a pass of 32 rows or more (1 = every CTA on one barrier); WB200_MK_TURNS: partitions that may
+        // stream cross K/V at the same time.  Defaults: what measured fastest at 64 rows (DESIGN.md section 4)
+        if (const char * np = getenv("WB200_MK_PARTS")) mk_parts = std::min(std::max(atoi(np), 1), MK_MAX_PARTS);
+        if (const char * ts = getenv("WB200_MK_TURNS")) mk_turns = std::min(std::max(atoi(ts), 1), MK_MAX_PARTS);
         sm_ghz = prop.clockRate * 1e-6;
         if (const char * tp = getenv("WB200_MK_TRACE")) { if (use_mk && *tp) { mk_trace_path = tp; if (!mk_trace.alloc(4096, true)) return false; } }
     }
@@ -175,11 +173,12 @@ void Engine::mk_trace_collect(int n_layer, bool logits) {
             for (int g = 0; g < 6; ++g) for (int k = 0; k < 5; ++k) mk_fine[5 * g + k] += (double) (f[8 * g + k + 1] - f[8 * g + k]);
         }
     }
-    ++mk_trace_n;
-    if (mk_gen == 2) {                                            // per-group time stamps of this pass (globaltimer, ns): layer start, cross-attention start / end
-        mk_gtrace.assign(3 * 4 * n_layer, 0);
-        cudaMemcpy(mk_gtrace.data(), mk_trace.p + 3000, mk_gtrace.size() * sizeof(long long), cudaMemcpyDeviceToHost);
+    {   // SM clocks the CTA that releases partition 0 waited for the partition's turn to stream cross K/V (the kernel accumulates)
+        long long w = 0;
+        if (cudaMemcpy(&w, mk_trace.p + 2100, sizeof(w), cudaMemcpyDeviceToHost) == cudaSuccess) mk_turn_clk += (double) w / n_layer;
+        cudaMemset(mk_trace.p + 2100, 0, sizeof(long long));
     }
+    ++mk_trace_n;
 }
 void Engine::mk_trace_dump() {
     if (mk_trace_path.empty() || !mk_trace_n) return;
@@ -199,16 +198,7 @@ void Engine::mk_trace_dump() {
         fprintf(f, "GEMV sub-phases, layer 1 (us): stage rows | k-loop of the first iteration | partials->smem + sync | epilogue + sync | remaining iterations\n");
         for (int g = 0; g < 6; ++g) fprintf(f, "  %-8s %7.2f %7.2f %7.2f %7.2f %7.2f\n", gn[g], mk_fine[5*g] * us, mk_fine[5*g+1] * us, mk_fine[5*g+2] * us, mk_fine[5*g+3] * us, mk_fine[5*g+4] * us);
     }
-    if (!mk_gtrace.empty()) {
-        fprintf(f, "row groups of the last traced pass (us since the first stamp): layer | per group: layer start, cross-attention start - end\n");
-        long long t0 = 0; for (long long v : mk_gtrace) if (v && (!t0 || v < t0)) t0 = v;
-        const int nl = (int) mk_gtrace.size() / 12;
-        for (int l = 0; l < nl; ++l) if (l < 6 || l >= nl - 2) {
-            fprintf(f, "  L%-2d", l);
-            for (int g = 0; g < 4; ++g) { const long long * v = &mk_gtrace[(l * 4 + g) * 3]; if (v[0]) fprintf(f, " | %8.1f %8.1f-%8.1f", (v[0] - t0) * 1e-3, (v[1] - t0) * 1e-3, (v[2] - t0) * 1e-3); }
-            fprintf(f, "\n");
-        }
-    }
+    fprintf(f, "partitions %d, turns %d: wait of partition 0 for its turn to stream cross K/V %.2f us per layer (inside the barrier of 6 cross-q)\n", mk_parts, mk_turns, mk_turn_clk * us);
     fprintf(f, "layer total %.2f us; final ln %.2f + barrier %.2f us, logits %.2f us; whole pass %.1f us\n", tot, mk_trace_sum[24] * us, mk_trace_sum[25] * us, mk_trace_sum[26] * us, mk_trace_sum[27] * us);
     fclose(f);
 }
@@ -488,31 +478,27 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         a.actq = reinterpret_cast<uint8_t *>(dattn.p); a.h = dh.p; a.hq = dhq.p;
         a.xpart = xpart.p; a.xcnt = xcnt.p;
         if (pass_capture) { a.cap = dtw_q.p; a.cap_row = d_cap; a.cap_rows = dtw_cap_rows; }
-        const int gen = (mk_gen == 2 && !pass_capture) ? 2 : 1;      // DTW capture exists in generation 1 only
-        if (mk_last_gen != 0 && gen != mk_last_gen) {                // the generations lay their barrier words out differently: start from zero
-            WB_CUDA_OK(cudaMemsetAsync(mk_bar.p, 0, mk_bar.bytes(), st));
-            mk_bar_total = 0;
-        }
-        mk_last_gen = gen;
         a.bar = mk_bar.p; a.bar_base = mk_bar_total; a.err = reinterpret_cast<int *>(mk_bar.p + 8); a.prefetch = mk_prefetch; a.trace = mk_trace.p;
-        if (gen == 2) {
-            // does a row attend to a self-KV cell that a row of ANOTHER 16-row group appends in this pass (several tokens of one sequence)?
-            a.stagger_clk = mk_stagger_clk;
-            if (n > 16) {
-                if (cell_group.size() < (size_t) n_cells) cell_group.assign(n_cells, 0);
-                ++cell_stamp;
-                if ((cell_stamp & 0xffffff) == 0) { std::fill(cell_group.begin(), cell_group.end(), 0u); cell_stamp = 1; }
-                const int * h_cell = hints + 2 * R, * h_nkv = hints + 4 * R, * h_idx = hints + 8 * R;
-                for (int t = 0; t < n; ++t) cell_group[h_cell[t]] = (cell_stamp << 8) | (uint32_t) (t >> 4);
-                for (int t = 0; t < n && !a.global_sync; ++t) {
-                    const int * row = h_idx + (size_t) t * ld_idx;
-                    for (int k = 0; k < h_nkv[t]; ++k) {
-                        const uint32_t cgv = cell_group[row[k]];
-                        if ((cgv >> 8) == cell_stamp && (int) (cgv & 0xff) != (t >> 4)) { a.global_sync = 1; break; }
-                    }
+        // A pass of 32 rows or more is cut into partitions unless a row attends to a self-KV cell that a row of ANOTHER 16-row group appends
+        // in this pass (several tokens of one sequence: prompt and DTW passes): those stay on one barrier.
+        if (n >= 32 && mk_parts > 1) {
+            if (cell_group.size() < (size_t) n_cells) cell_group.assign(n_cells, 0);
+            ++cell_stamp;
+            if ((cell_stamp & 0xffffff) == 0) { std::fill(cell_group.begin(), cell_group.end(), 0u); cell_stamp = 1; }
+            const int * h_cell = hints + 2 * R, * h_nkv = hints + 4 * R, * h_idx = hints + 8 * R;
+            for (int t = 0; t < n; ++t) cell_group[h_cell[t]] = (cell_stamp << 8) | (uint32_t) (t >> 4);
+            bool shared = false;
+            for (int t = 0; t < n && !shared; ++t) {
+                const int * row = h_idx + (size_t) t * ld_idx;
+                for (int k = 0; k < h_nkv[t]; ++k) {
+                    const uint32_t cgv = cell_group[row[k]];
+                    if ((cgv >> 8) == cell_stamp && (int) (cgv & 0xff) != (t >> 4)) { shared = true; break; }
                 }
             }
+            if (!shared) a.n_part = std::min(mk_parts, (n + 15) / 16);
         }
+        a.turn_slots = mk_turns;
+        std::copy(mk_bar_part, mk_bar_part + MK_MAX_PARTS, a.part_base);
         // algorithmic bytes of one pass: every decoder weight once, the cross K/V of each row, the self K/V each row attends to
         double wbytes = 0.0, flops = 0.0;
         for (int l = 0; l < Lt; ++l) {
@@ -524,13 +510,10 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         for (int j = 0; j < n; ++j) kvbytes += (double) Lt * 2.0 * d * 2.0 * ((double) n_keys + hints[4 * R + j]);
         flops += kvbytes;                                           // 2 flops per KV element (f16 = 2 bytes): same number
         ProfScope prof(PC_GEMV, st, wbytes + kvbytes, flops);
-        if (gen == 2) {
-            if (!mk2_launch(a, m->wtype == WT_F32 ? WT_F16 : m->wtype, n_sm, st)) return false;
-            mk_bar_total += 4096;
-        } else {
-            if (!mk_launch(a, m->wtype == WT_F32 ? WT_F16 : m->wtype, n_sm, st)) return false;
-            mk_bar_total += (unsigned long long) n_sm * mk_barriers(m->wtype == WT_F32 ? WT_F16 : m->wtype, Lt, any_logits);
-        }
+        if (!mk_launch(a, m->wtype == WT_F32 ? WT_F16 : m->wtype, n_sm, st)) return false;
+        for (int p = 0; p < a.n_part; ++p)
+            mk_bar_part[p] += (unsigned long long) mk_partition(p, a.n_part, n_sm, n).nc * mk_layer_barriers(m->wtype == WT_F32 ? WT_F16 : m->wtype) * Lt;
+        if (any_logits) mk_bar_total += (unsigned long long) n_sm;
     } else
     for (int l = 0; l < Lt; ++l) {
         const DecLayerW & L = m->dec[l];

@@ -82,19 +82,17 @@ struct Engine {
     bool dtw_weights(const std::vector<int> & req, std::vector<std::vector<float> *> & out);
     bool use_mk = false;
     int  max_rows = 8;               // rows per decode pass: 64 with the persistent kernel, 8 with the chain
-    int  n_sm = 0, mk_prefetch = 61;     // bit0: next-phase weights -> L2; bit2: K / V streams with L2 evict-first priority; bit3 (generation 2): row groups take turns in the cross-attention; bit4: logits one warp per weight tile
+    int  n_sm = 0, mk_prefetch = 61;     // bit0: next-phase weights -> L2; bit2: K / V streams with L2 evict-first priority; bit4: logits one warp per weight tile
     DevBuf<MkLayer> mk_layers;
-    DevBuf<unsigned long long> mk_bar;   // [0] arrival counter, [8] error flag, [16 + 16*cta] release flags
-    unsigned long long mk_bar_total = 0;
-    int mk_gen = 1, mk_stagger_clk = 0;              // kernel generation (wb_decode_mk2.cu = 2), start stagger of its row groups
+    DevBuf<unsigned long long> mk_bar;   // barrier words of the persistent kernel (mk_bar_words)
+    unsigned long long mk_bar_total = 0, mk_bar_part[MK_MAX_PARTS] = {};   // arrivals so far at the grid's counter and at the partitions' counters
+    int mk_parts = 4, mk_turns = 2;      // partitions of a pass of 32 rows or more; partitions that may stream cross K/V at the same time
     std::vector<uint32_t> cell_group; uint32_t cell_stamp = 0;   // host scratch: which row group appends a cell in the current pass
     bool mk_build_table();
     // WB200_MK_TRACE=<file>: per-phase clock stamps of CTA 0, averaged over all passes, written when the engine is destroyed
-    DevBuf<long long> mk_trace; std::vector<double> mk_trace_sum, mk_fine; uint64_t mk_trace_n = 0; std::string mk_trace_path; double sm_ghz = 1.0;
-    std::vector<long long> mk_gtrace;
+    DevBuf<long long> mk_trace; std::vector<double> mk_trace_sum, mk_fine; uint64_t mk_trace_n = 0; double mk_turn_clk = 0.0; std::string mk_trace_path; double sm_ghz = 1.0;
     void mk_trace_collect(int n_layer, bool logits);
     void mk_trace_dump();
-    int mk_last_gen = 0;             // generation of the last launch: the two keep different barrier words (reset when they alternate)
     DevBuf<int>    dints, xcnt;      // packed per-step integers: tokens | pos | cells | slot | n_kv | rowinfo[2] | capture index | idx[...]
     DevBuf<uint32_t> samp_mask;      // static suppression bit mask of the on-device sampler
     uint64_t samp_mask_key = 0;
