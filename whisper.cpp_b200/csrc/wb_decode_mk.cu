@@ -147,6 +147,15 @@ __device__ __noinline__ void mk_grid_sync(const MkArgs & a, const MkView v, unsi
 // less than a super-block (attention heads, FC1 tiles) write f32 rows, and a quantise phase (mk_q8k_rows) follows them.
 constexpr bool mk_kq(int WT) { return WT == WT_Q4_K || WT == WT_Q5_K; }
 
+// Q4_1 / Q5_1 weights: rows are Q8_1 (quantize_row_q8_1, AVX2 form ggml-cpu/arch/x86/quants.c): the int8 values of Q8_0 (with the IEEE
+// quotients 127/amax and amax/127 the reference uses), and in place of each f32 block scale the pair {f16 d, f16 s = d * sum(q)} (s from
+// the unrounded d) -- same bytes per row, so staging and workspaces are those of Q8_0.  The block dot is (d_w d_x) sumi + m_w s_x.
+constexpr bool mk_q1(int WT) { return WT == WT_Q4_1 || WT == WT_Q5_1; }
+__device__ __forceinline__ uint32_t q8_1_pair(float d, int sum) {
+    const __half2 p = __halves2half2(__float2half_rn(d), __float2half_rn(d * (float) sum));
+    return *reinterpret_cast<const uint32_t *>(&p);
+}
+
 // the signed value of largest magnitude of two candidates; ties go to the larger value, so the choice does not depend on the order
 // (a tie between x and -x only flips the signs of q and d together)
 __device__ __forceinline__ void q8k_pick(float & amax, float & mx, float oa, float om) {
@@ -177,10 +186,27 @@ template <int WT>
 __device__ __forceinline__ void mk_store_q(uint8_t * dst, int K, int t, int e0, int lane, float v) {
     if (WT == WT_F16) { reinterpret_cast<__half *>(dst)[(size_t) t * K + e0 + lane] = __float2half_rn(v); return; }
     if (mk_kq(WT)) { reinterpret_cast<float *>(dst)[(size_t) t * K + e0 + lane] = v; return; }
+    if (mk_q1(WT)) {
+        const float amax = warp_max(fabsf(v));
+        const int q = __float2int_rn(v * ((amax != 0.0f) ? 127.0f / amax : 0.0f));
+        reinterpret_cast<int8_t *>(dst)[(size_t) t * K + e0 + lane] = (int8_t) q;
+        const int sum = __reduce_add_sync(0xffffffffu, q);
+        if (lane == 0) reinterpret_cast<uint32_t *>(dst + (size_t) MK_MAXTOK * K)[t * (K >> 5) + (e0 >> 5)] = q8_1_pair(amax / 127.0f, sum);
+        return;
+    }
     const float amax = warp_max(fabsf(v));
     const float id = (amax != 0.0f) ? __fdividef(127.0f, amax) : 0.0f;
     reinterpret_cast<int8_t *>(dst)[(size_t) t * K + e0 + lane] = (int8_t) __float2int_rn(v * id);
     if (lane == 0) reinterpret_cast<float *>(dst + (size_t) MK_MAXTOK * K)[t * (K >> 5) + (e0 >> 5)] = __half2float(__float2half_rn(amax * (1.0f / 127.0f)));
+}
+
+// Q8_1 of four values per lane, 8 lanes per 32-value block (amax already reduced over the 8 lanes)
+__device__ __forceinline__ void mk_q8_1_store4(uint8_t * dst, int K, int row, int e0, int lane, const float4 & y, float amax) {
+    const float id = (amax != 0.0f) ? 127.0f / amax : 0.0f;
+    const int q0 = __float2int_rn(y.x * id), q1 = __float2int_rn(y.y * id), q2 = __float2int_rn(y.z * id), q3 = __float2int_rn(y.w * id);
+    *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0) = ((uint32_t) q0 & 0xffu) | (((uint32_t) q1 & 0xffu) << 8) | (((uint32_t) q2 & 0xffu) << 16) | ((uint32_t) q3 << 24);
+    const int sum = sum8_lanes((q0 + q1) + (q2 + q3));
+    if ((lane & 7) == 0) reinterpret_cast<uint32_t *>(dst + (size_t) MK_MAXTOK * K)[row * (K >> 5) + (e0 >> 5)] = q8_1_pair(amax / 127.0f, sum);
 }
 
 // LayerNorm (ggml-cpu/ops.cpp:3698-3765, two passes, then mul/add whisper.cpp:2536-2543) of the f32 residual rows, quantised into
@@ -245,11 +271,13 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const MkView v, const floa
                 amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
                 amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
                 amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
+                if (mk_q1(WT)) { mk_q8_1_store4(dst, K, row, e0, lane, y, amax); } else {
                 const float id = (amax != 0.0f) ? __fdividef(127.0f, amax) : 0.0f;
                 const uint32_t q0 = (uint32_t) __float2int_rn(y.x * id) & 0xffu, q1 = (uint32_t) __float2int_rn(y.y * id) & 0xffu;
                 const uint32_t q2 = (uint32_t) __float2int_rn(y.z * id) & 0xffu, q3 = (uint32_t) __float2int_rn(y.w * id) & 0xffu;
                 *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0) = q0 | (q1 << 8) | (q2 << 16) | (q3 << 24);
                 if ((lane & 7) == 0) reinterpret_cast<float *>(dst + (size_t) MK_MAXTOK * K)[row * (K >> 5) + (e0 >> 5)] = __half2float(__float2half_rn(amax * (1.0f / 127.0f)));
+                }
             }
         }
         __syncthreads();
@@ -274,11 +302,13 @@ __device__ __noinline__ void mk_q8_rows(const MkView v, const float * src, int K
             amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
             amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
             amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
+            if (mk_q1(WT)) { mk_q8_1_store4(dst, K, row, e0, lane, y, amax); } else {
             const float id = (amax != 0.0f) ? __fdividef(127.0f, amax) : 0.0f;
             const uint32_t q0 = (uint32_t) __float2int_rn(y.x * id) & 0xffu, q1 = (uint32_t) __float2int_rn(y.y * id) & 0xffu;
             const uint32_t q2 = (uint32_t) __float2int_rn(y.z * id) & 0xffu, q3 = (uint32_t) __float2int_rn(y.w * id) & 0xffu;
             *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0) = q0 | (q1 << 8) | (q2 << 16) | (q3 << 24);
             if ((lane & 7) == 0) reinterpret_cast<float *>(dst + (size_t) MK_MAXTOK * K)[row * (K >> 5) + (e0 >> 5)] = __half2float(__float2half_rn(amax * (1.0f / 127.0f)));
+            }
         }
         row += drow; ch += dch; if (ch >= cpr) { ch -= cpr; ++row; }
     }
@@ -343,8 +373,9 @@ __device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_all;
 // 2.4 us for three slots): an iteration with four slots makes two calls of two slots, same partials, no spills.
 template <int WT, int NV, int TU, int KS, int UB>
 __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * wbase, int tile0, int tstep, int nrec, int nb, int SW, int nt, int NH, bool & staged, uint32_t stage_parity, int fb, int j0) {
-    constexpr bool KQ = mk_kq(WT);
-    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 : 512));   // K-quants: bytes per 32 values
+    constexpr bool KQ = mk_kq(WT), Q1 = mk_q1(WT);
+    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
+                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : 512))));   // K-quants: bytes per 32 values
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RLD = 17;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3, ks = warp & (KS - 1);
@@ -354,7 +385,7 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 #pragma unroll
         for (int h = 0; h < 2; ++h) { acc[j][h][0] = acc[j][h][1] = acc[j][h][2] = acc[j][h][3] = 0.0f; }
     for (int kb = ks; kb < nrec; kb += KS * UB) {
-        uint4 wq[NV][UB]; uint2 wh[NV][UB]; uint32_t wd[NV][UB]; uint2 wk[NV][UB];
+        uint4 wq[NV][UB]; uint2 wh[NV][UB]; uint32_t wd[NV][UB]; uint2 wk[NV][UB]; uint2 wm[NV][UB];
 #pragma unroll
         for (int j = 0; j < NV; ++j) {
             {
@@ -372,8 +403,9 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                     const uint8_t * rec = tb + (size_t) min(kb + u * KS, nrec - 1) * REC;
                     if (WT == WT_F16 || WT == WT_Q8_0) wq[j][u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
                     else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[j][u].x = q2.x; wq[j][u].y = q2.y; }
-                    if (WT == WT_Q5_0) wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
-                    if (WT != WT_F16)  wd[j][u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
+                    if (WT == WT_Q5_0 || WT == WT_Q5_1) wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
+                    if (Q1) wm[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB + (WT == WT_Q5_1 ? 64 : 0)) + g);   // {d, d'}, {m, m'}
+                    else if (WT != WT_F16)  wd[j][u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
                 }
             }
         }
@@ -394,6 +426,10 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                         dx[h][0] = SM_XD[r0 * nb + (b >> 3)]; dx[h][1] = SM_XD[r1 * nb + (b >> 3)];
                         sx[h][0] = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
                         sx[h][1] = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+                    } else if (Q1) {                             // Q8_1: {d, s} of the block
+                        const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c, nt - 1) * nb + b];
+                        const __half2 p1 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
+                        dx[h][0] = __low2float(p0); sx[h][0] = __high2float(p0); dx[h][1] = __low2float(p1); sx[h][1] = __high2float(p1);
                     } else if (WT != WT_F16) { dx[h][0] = SM_XD[min(h * 8 + 2 * c, nt - 1) * nb + b]; dx[h][1] = SM_XD[min(h * 8 + 2 * c + 1, nt - 1) * nb + b]; }
                 }
 #pragma unroll
@@ -416,6 +452,30 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                                 acc[j][h][1] = fmaf(dx[h][1], fmaf(dl0, (float) dd[1], -ml0 * sx[h][1]), acc[j][h][1]);
                                 acc[j][h][2] = fmaf(dx[h][0], fmaf(dl1, (float) dd[2], -ml1 * sx[h][0]), acc[j][h][2]);
                                 acc[j][h][3] = fmaf(dx[h][1], fmaf(dl1, (float) dd[3], -ml1 * sx[h][1]), acc[j][h][3]);
+                            }
+                        }
+                        continue;
+                    }
+                    if (Q1) {                                    // unsigned 4 / 5-bit weights; acc += (d_w d_x) sumi, then m_w s_x
+                        uint32_t af[4];
+                        af[0] = wq[j][u].x & 0x0F0F0F0Fu; af[2] = (wq[j][u].x >> 4) & 0x0F0F0F0Fu;
+                        af[1] = wq[j][u].y & 0x0F0F0F0Fu; af[3] = (wq[j][u].y >> 4) & 0x0F0F0F0Fu;
+                        if (WT == WT_Q5_1) {
+                            af[0] |= spread4_to_bit4(wh[j][u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[j][u].x >> (16 + 4 * c));
+                            af[1] |= spread4_to_bit4(wh[j][u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[j][u].y >> (16 + 4 * c));
+                        }
+                        const float dw0 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].x & 0xffffu)));
+                        const float dw1 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].x >> 16)));
+                        const float mw0 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].y & 0xffffu)));
+                        const float mw1 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].y >> 16)));
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            if (h < NH) {
+                                int dd[4]; mma_s8_16832(dd, af, bf[h][0], bf[h][1]);
+                                acc[j][h][0] = fmaf(mw0, sx[h][0], fmaf(dw0 * dx[h][0], (float) dd[0], acc[j][h][0]));
+                                acc[j][h][1] = fmaf(mw0, sx[h][1], fmaf(dw0 * dx[h][1], (float) dd[1], acc[j][h][1]));
+                                acc[j][h][2] = fmaf(mw1, sx[h][0], fmaf(dw1 * dx[h][0], (float) dd[2], acc[j][h][2]));
+                                acc[j][h][3] = fmaf(mw1, sx[h][1], fmaf(dw1 * dx[h][1], (float) dd[3], acc[j][h][3]));
                             }
                         }
                         continue;
@@ -484,7 +544,6 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 // quantised-row format FC2 consumes (one warp = one Q8_0 block of one row) -- no f32 round trip, no extra phase.
 template <int WT, bool PAIR>
 __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, const MkEpi & e, int fb = -1) {
-    constexpr int REC = (WT == WT_Q4_0) ? 288 : (WT == WT_Q5_0 ? 352 : (WT == WT_Q8_0 ? 544 : 512));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;             // bytes of the qs part of a record
     constexpr int RK = (WT == WT_F16) ? 16 : 32;                 // K values per record
     constexpr int UB = 3;                                        // records whose loads are issued together
@@ -530,7 +589,7 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
                 case 1: if (!PAIR) { mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
                 case 2: mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break;
                 case 3:
-                    if (!PAIR && mk_kq(WT)) {                    // K-quant records carry a header share (and Q5_K fifth bits): two slots + one
+                    if (!PAIR && (mk_kq(WT) || WT == WT_Q5_1)) {     // K-quant records carry a header share (and Q5_K fifth bits), Q5_1 ones fifth bits and minima: two slots + one
                         mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0);
                         mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 2);
                         break;
@@ -599,8 +658,9 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
 // is one accumulator over the blocks in ascending order: independent of the batch.
 template <int WT>
 __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, float * out) {
-    constexpr bool KQ = mk_kq(WT);
-    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 : 512));
+    constexpr bool KQ = mk_kq(WT), Q1 = mk_q1(WT);
+    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
+                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : 512))));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RK = (WT == WT_F16) ? 16 : 32;
     constexpr int UB = 8;
@@ -636,7 +696,7 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
         for (int h = 0; h < 2; ++h) { acc[h][0] = acc[h][1] = acc[h][2] = acc[h][3] = 0.0f; }
         const uint8_t * tb = wbase + (size_t) tile * nrec * REC;
         for (int kb = 0; kb < nrec; kb += UB) {
-            uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB]; uint2 wk[UB];
+            uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB]; uint2 wk[UB]; uint2 wm[UB];
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
                 if (KQ) {
@@ -650,8 +710,9 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
                 const uint8_t * rec = tb + (size_t) min(kb + u, nrec - 1) * REC;
                 if (WT == WT_F16 || WT == WT_Q8_0) wq[u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
                 else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[u].x = q2.x; wq[u].y = q2.y; }
-                if (WT == WT_Q5_0) wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
-                if (WT != WT_F16)  wd[u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
+                if (WT == WT_Q5_0 || WT == WT_Q5_1) wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
+                if (Q1) wm[u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB + (WT == WT_Q5_1 ? 64 : 0)) + g);
+                else if (WT != WT_F16)  wd[u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
             }
             if (!staged) { mbar_wait(SM_MBAR, stage_parity); staged = true; }
 #pragma unroll
@@ -683,7 +744,33 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
                             acc[h][3] = fmaf(dx1, fmaf(dl1, (float) dd[3], -ml1 * sx1), acc[h][3]);
                         }
                     }
-                } else if (!KQ && b < nrec) {
+                } else if (Q1 && b < nrec) {
+                    uint32_t af[4];
+                    af[0] = wq[u].x & 0x0F0F0F0Fu; af[2] = (wq[u].x >> 4) & 0x0F0F0F0Fu;
+                    af[1] = wq[u].y & 0x0F0F0F0Fu; af[3] = (wq[u].y >> 4) & 0x0F0F0F0Fu;
+                    if (WT == WT_Q5_1) {
+                        af[0] |= spread4_to_bit4(wh[u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[u].x >> (16 + 4 * c));
+                        af[1] |= spread4_to_bit4(wh[u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[u].y >> (16 + 4 * c));
+                    }
+                    const float dw0 = __half2float(__ushort_as_half((unsigned short) (wm[u].x & 0xffffu)));
+                    const float dw1 = __half2float(__ushort_as_half((unsigned short) (wm[u].x >> 16)));
+                    const float mw0 = __half2float(__ushort_as_half((unsigned short) (wm[u].y & 0xffffu)));
+                    const float mw1 = __half2float(__ushort_as_half((unsigned short) (wm[u].y >> 16)));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (h < NH) {
+                            const bool ok = h * 8 + g < nt;
+                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
+                            const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c, nt - 1) * nb + b];
+                            const __half2 p1 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
+                            int dd[4]; mma_s8_16832(dd, af, b0, b1);
+                            acc[h][0] = fmaf(mw0, __high2float(p0), fmaf(dw0 * __low2float(p0), (float) dd[0], acc[h][0]));
+                            acc[h][1] = fmaf(mw0, __high2float(p1), fmaf(dw0 * __low2float(p1), (float) dd[1], acc[h][1]));
+                            acc[h][2] = fmaf(mw1, __high2float(p0), fmaf(dw1 * __low2float(p0), (float) dd[2], acc[h][2]));
+                            acc[h][3] = fmaf(mw1, __high2float(p1), fmaf(dw1 * __low2float(p1), (float) dd[3], acc[h][3]));
+                        }
+                    }
+                } else if (!KQ && !Q1 && b < nrec) {
                     uint32_t af[4];
                     float dw0 = 0.0f, dw1 = 0.0f;
                     if (WT == WT_F16 || WT == WT_Q8_0) { af[0] = wq[u].x; af[1] = wq[u].y; af[2] = wq[u].z; af[3] = wq[u].w; }
@@ -1131,6 +1218,8 @@ bool mk_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st) {
         case WT_F16:  return WB_MK(WT_F16);
         case WT_Q4_0: return WB_MK(WT_Q4_0);
         case WT_Q5_0: return WB_MK(WT_Q5_0);
+        case WT_Q4_1: return WB_MK(WT_Q4_1);
+        case WT_Q5_1: return WB_MK(WT_Q5_1);
         case WT_Q8_0: return WB_MK(WT_Q8_0);
         case WT_Q4_K: return WB_MK(WT_Q4_K);
         case WT_Q5_K: return WB_MK(WT_Q5_K);

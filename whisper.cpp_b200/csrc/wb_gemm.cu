@@ -43,7 +43,7 @@ struct GemmKParams {
     int n_mt, n_nt, n_tiles;        // tile list: weight tile fastest, then activation tile, then batch index
     int b_split;                    // 2: the B tensor map's box holds BN / 2 rows (the tile is fetched in two halves)
     // quantised A
-    const void * a_base; const uint8_t * a_qs; const uint32_t * a_qh; const __half * a_d;
+    const void * a_base; const uint8_t * a_qs; const uint32_t * a_qh; const __half * a_d; const __half * a_m;
     GemmEpilogue ep;
 };
 
@@ -59,17 +59,18 @@ __device__ __forceinline__ float gelu_ref_f16(float x) {
     return __half2float(__float2half_rn(__fdividef(xh, 1.0f + e)));
 }
 
-struct RawBlk { uint4 q0, q1; uint32_t qh; __half d; };
+struct RawBlk { uint4 q0, q1; uint32_t qh; __half d, m; };
 
 template <int WT>
 __device__ __forceinline__ void raw_load(const GemmKParams & p, int m, int k, RawBlk & r, bool valid) {
     if (!valid) { r.q0 = r.q1 = make_uint4(0, 0, 0, 0); r.qh = 0; r.d = __float2half(0.0f); return; }
     const int64_t nblk = (int64_t) p.K >> 5;
     const int64_t bi   = (int64_t) m * nblk + (k >> 5);
-    if (WT == WT_Q4_0 || WT == WT_Q5_0) {
+    if (WT == WT_Q4_0 || WT == WT_Q5_0 || WT == WT_Q4_1 || WT == WT_Q5_1) {
         r.q0 = __ldg(reinterpret_cast<const uint4 *>(p.a_qs) + bi);
-        if (WT == WT_Q5_0) r.qh = __ldg(p.a_qh + bi);
+        if (wt_has_qh(WT)) r.qh = __ldg(p.a_qh + bi);
         r.d = p.a_d[bi];
+        if (wt_has_min(WT)) r.m = p.a_m[bi];
     } else if (WT == WT_Q8_0) {
         r.q0 = __ldg(reinterpret_cast<const uint4 *>(p.a_qs) + 2*bi);
         r.q1 = __ldg(reinterpret_cast<const uint4 *>(p.a_qs) + 2*bi + 1);
@@ -370,6 +371,8 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
                             raw_load<WT>(p, m, k, rb, true);
                             if (WT == WT_Q4_0)      dequant_q4_0(rb.q0, rb.d, q);
                             else if (WT == WT_Q5_0) dequant_q5_0(rb.q0, rb.qh, rb.d, q);
+                            else if (WT == WT_Q4_1) dequant_q4_1(rb.q0, rb.d, rb.m, q);
+                            else if (WT == WT_Q5_1) dequant_q5_1(rb.q0, rb.qh, rb.d, rb.m, q);
                             else                    dequant_q8_0(rb.q0, rb.q1, rb.d, q);
                             oh[0] = q[0]; oh[1] = q[1]; oh[2] = q[2]; oh[3] = q[3];
                         }
@@ -427,7 +430,7 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
 // Each value is the f16 rounding of the exact d * (q - off), i.e. what dequantize_row_* gives after one f16 store (wb_quant.cuh).
 template <int WT>
 __global__ void __launch_bounds__(256)
-k_dequant_f16(const void * base, const uint8_t * qs, const uint32_t * qh, const __half * dd, int64_t row0, int64_t n_blocks, int K, __half * out) {
+k_dequant_f16(const void * base, const uint8_t * qs, const uint32_t * qh, const __half * dd, const __half * mm, int64_t row0, int64_t n_blocks, int K, __half * out) {
     const int64_t bi = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (bi >= n_blocks) return;
     const int64_t nblk = K >> 5;
@@ -441,6 +444,8 @@ k_dequant_f16(const void * base, const uint8_t * qs, const uint32_t * qh, const 
         const int64_t g = row0 * nblk + bi;
         if (WT == WT_Q4_0)      dequant_q4_0(__ldg(reinterpret_cast<const uint4 *>(qs) + g), dd[g], o);
         else if (WT == WT_Q5_0) dequant_q5_0(__ldg(reinterpret_cast<const uint4 *>(qs) + g), __ldg(qh + g), dd[g], o);
+        else if (WT == WT_Q4_1) dequant_q4_1(__ldg(reinterpret_cast<const uint4 *>(qs) + g), dd[g], mm[g], o);
+        else if (WT == WT_Q5_1) dequant_q5_1(__ldg(reinterpret_cast<const uint4 *>(qs) + g), __ldg(qh + g), dd[g], mm[g], o);
         else                    dequant_q8_0(__ldg(reinterpret_cast<const uint4 *>(qs) + 2*g), __ldg(reinterpret_cast<const uint4 *>(qs) + 2*g + 1), dd[g], o);
     }
     uint4 * dst = reinterpret_cast<uint4 *>(out + bi * 32);
@@ -537,11 +542,13 @@ cudaError_t dequant_to_f16(const QMat & W, int64_t rows, __half * out, cudaStrea
     const int64_t n_blocks = rows * (W.K >> 5);
     const unsigned grid = (unsigned) ((n_blocks + 255) / 256);
     switch (W.type) {
-        case WT_Q4_0: k_dequant_f16<WT_Q4_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, 0, n_blocks, W.K, out); break;
-        case WT_Q5_0: k_dequant_f16<WT_Q5_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, 0, n_blocks, W.K, out); break;
-        case WT_Q8_0: k_dequant_f16<WT_Q8_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, 0, n_blocks, W.K, out); break;
-        case WT_Q4_K: k_dequant_f16<WT_Q4_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, 0, n_blocks, W.K, out); break;
-        case WT_Q5_K: k_dequant_f16<WT_Q5_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, 0, n_blocks, W.K, out); break;
+        case WT_Q4_0: k_dequant_f16<WT_Q4_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q4_1: k_dequant_f16<WT_Q4_1><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q5_0: k_dequant_f16<WT_Q5_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q5_1: k_dequant_f16<WT_Q5_1><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q8_0: k_dequant_f16<WT_Q8_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q4_K: k_dequant_f16<WT_Q4_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q5_K: k_dequant_f16<WT_Q5_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
         default: return cudaErrorInvalidValue;
     }
     count_launch();
@@ -563,7 +570,7 @@ cudaError_t gemm_launch(const GemmDesc & g, cudaStream_t st) {
     kp.M = g.M; kp.N = g.N; kp.K = g.K; kp.taps = g.taps; kp.nkb_per_tap = (g.K + 63) / 64; kp.nb0 = g.nb0;
     kp.a_zsel0 = g.a_zsel[0]; kp.a_zsel1 = g.a_zsel[1]; kp.b_zsel0 = g.b_zsel[0]; kp.b_zsel1 = g.b_zsel[1];
     kp.a_rows_per_b0 = g.a_rows_per_b0; kp.b1_in_off = g.b1_in_off;
-    kp.a_base = g.A.base; kp.a_qs = g.A.qs; kp.a_qh = g.A.qh; kp.a_d = g.A.d;
+    kp.a_base = g.A.base; kp.a_qs = g.A.qs; kp.a_qh = g.A.qh; kp.a_d = g.A.d; kp.a_m = g.A.m;
     kp.ep = g.ep;
     kp.b_split = g.half_box_b ? 2 : 1;
     if (g.half_box_b && g.BN < 128) return cudaErrorInvalidValue;
@@ -575,6 +582,8 @@ cudaError_t gemm_launch(const GemmDesc & g, cudaStream_t st) {
         case WT_F16:  return launch_ek<WT_F16>(g, kp, false, st);
         case WT_Q4_0: return launch_ek<WT_Q4_0>(g, kp, false, st);
         case WT_Q5_0: return launch_ek<WT_Q5_0>(g, kp, false, st);
+        case WT_Q4_1: return launch_ek<WT_Q4_1>(g, kp, false, st);
+        case WT_Q5_1: return launch_ek<WT_Q5_1>(g, kp, false, st);
         case WT_Q8_0: return launch_ek<WT_Q8_0>(g, kp, false, st);
         case WT_Q4_K: return launch_ek<WT_Q4_K>(g, kp, false, st);
         case WT_Q5_K: return launch_ek<WT_Q5_K>(g, kp, false, st);

@@ -40,15 +40,16 @@ void f16_to_f32(const __half * src, float * dst, int64_t n, cudaStream_t st) {
 // one thread per 32-block: gather the unaligned file block with byte loads, scatter to the planar arrays
 template <int WT>
 __global__ void k_repack32(const uint8_t * __restrict__ src, uint8_t * __restrict__ qs, uint32_t * __restrict__ qh,
-                           __half * __restrict__ d, int64_t nblk) {
-    constexpr int BS = (WT == WT_Q4_0) ? 18 : (WT == WT_Q5_0 ? 22 : 34);
+                           __half * __restrict__ d, __half * __restrict__ m, int64_t nblk) {
+    constexpr int BS = (WT == WT_Q4_0) ? 18 : (WT == WT_Q5_0 ? 22 : (WT == WT_Q4_1 ? 20 : (WT == WT_Q5_1 ? 24 : 34)));
     constexpr int QS = (WT == WT_Q8_0) ? 32 : 16;
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nblk) return;
     const uint8_t * b = src + i * BS;
     d[i] = __ushort_as_half((unsigned short) ((uint16_t) b[0] | ((uint16_t) b[1] << 8)));
     int off = 2;
-    if (WT == WT_Q5_0) { qh[i] = (uint32_t) b[2] | ((uint32_t) b[3] << 8) | ((uint32_t) b[4] << 16) | ((uint32_t) b[5] << 24); off = 6; }
+    if (wt_has_min(WT)) { m[i] = __ushort_as_half((unsigned short) ((uint16_t) b[2] | ((uint16_t) b[3] << 8))); off = 4; }
+    if (wt_has_qh(WT)) { qh[i] = (uint32_t) b[off] | ((uint32_t) b[off + 1] << 8) | ((uint32_t) b[off + 2] << 16) | ((uint32_t) b[off + 3] << 24); off += 4; }
     for (int j = 0; j < QS; ++j) qs[i * QS + j] = b[off + j];
 }
 bool repack_block32_into(int wtype, const uint8_t * src, const QMat & dst, int rows, int K, cudaStream_t st) {
@@ -56,10 +57,13 @@ bool repack_block32_into(int wtype, const uint8_t * src, const QMat & dst, int r
     if (nblk == 0) return true;
     const int blocks = (int) ((nblk + 255) / 256);
     uint8_t * qs = const_cast<uint8_t *>(dst.qs); uint32_t * qh = const_cast<uint32_t *>(dst.qh); __half * d = const_cast<__half *>(dst.d);
+    __half * m = const_cast<__half *>(dst.m);
     switch (wtype) {
-        case WT_Q4_0: k_repack32<WT_Q4_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, nblk); break;
-        case WT_Q5_0: k_repack32<WT_Q5_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, nblk); break;
-        case WT_Q8_0: k_repack32<WT_Q8_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, nblk); break;
+        case WT_Q4_0: k_repack32<WT_Q4_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, m, nblk); break;
+        case WT_Q4_1: k_repack32<WT_Q4_1><<<blocks, 256, 0, st>>>(src, qs, qh, d, m, nblk); break;
+        case WT_Q5_0: k_repack32<WT_Q5_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, m, nblk); break;
+        case WT_Q5_1: k_repack32<WT_Q5_1><<<blocks, 256, 0, st>>>(src, qs, qh, d, m, nblk); break;
+        case WT_Q8_0: k_repack32<WT_Q8_0><<<blocks, 256, 0, st>>>(src, qs, qh, d, m, nblk); break;
         default: set_error("repack_block32: bad type %d", wtype); return false;
     }
     count_launch();
@@ -70,8 +74,9 @@ bool repack_block32(int wtype, const uint8_t * src, uint8_t * dst, int N, int K,
     out->type = wtype; out->N = N; out->K = K; out->base = nullptr;
     out->qs = dst;
     uint8_t * p = dst + nblk * wt_qs_bytes(wtype);
-    out->qh = nullptr;
-    if (wtype == WT_Q5_0) { out->qh = reinterpret_cast<uint32_t *>(p); p += nblk * 4; }
+    out->qh = nullptr; out->m = nullptr;
+    if (wt_has_qh(wtype)) { out->qh = reinterpret_cast<uint32_t *>(p); p += nblk * 4; }
+    if (wt_has_min(wtype)) { out->m = reinterpret_cast<__half *>(p); p += nblk * 2; }
     out->d = reinterpret_cast<__half *>(p);
     return repack_block32_into(wtype, src, *out, N, K, st);
 }
@@ -79,7 +84,7 @@ bool repack_block32(int wtype, const uint8_t * src, uint8_t * dst, int N, int K,
 // tile-major records (wb_quant.cuh): one thread per (tile, record, lane)
 template <int WT>
 __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int rows, int K, int64_t n_threads) {
-    constexpr int BS = (WT == WT_Q4_0) ? 18 : (WT == WT_Q5_0 ? 22 : (WT == WT_Q8_0 ? 34 : 0));
+    constexpr int BS = (WT == WT_Q4_0) ? 18 : (WT == WT_Q5_0 ? 22 : (WT == WT_Q4_1 ? 20 : (WT == WT_Q5_1 ? 24 : (WT == WT_Q8_0 ? 34 : 0))));
     const int REC = wt_tm_rec_bytes(WT), nrec = K / wt_tm_rec_k(WT);
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_threads) return;
@@ -103,7 +108,7 @@ __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restri
         return;
     }
     const uint8_t * b0 = src + (r0 * nrec + b) * BS, * b1 = src + (r1 * nrec + b) * BS;
-    const int qoff = (WT == WT_Q5_0) ? 6 : 2;
+    const int qoff = (WT == WT_Q5_0) ? 6 : (WT == WT_Q4_1 ? 4 : (WT == WT_Q5_1 ? 8 : 2));
     auto word = [&](const uint8_t * blk, int64_t r, int wi) -> uint32_t {
         if (r >= rows) return 0u;
         const uint8_t * q = blk + qoff + 4 * wi;
@@ -114,7 +119,14 @@ __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restri
     if (c == 0) {                                                // lanes 0,4,..: the per-row fields of rows g and g+8
         const int qsb = (WT == WT_Q8_0) ? 512 : 256;
         auto d16 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[0] | ((uint32_t) blk[1] << 8)) : 0u; };
-        if (WT == WT_Q5_0) {
+        if (wt_has_min(WT)) {                                    // Q4_1 / Q5_1: file block d, m, (qh), qs
+            auto m16 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[2] | ((uint32_t) blk[3] << 8)) : 0u; };
+            if (WT == WT_Q5_1) {
+                auto h32 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[4] | ((uint32_t) blk[5] << 8) | ((uint32_t) blk[6] << 16) | ((uint32_t) blk[7] << 24)) : 0u; };
+                reinterpret_cast<uint2 *>(rec + qsb)[g] = make_uint2(h32(b0, r0), h32(b1, r1));
+            }
+            reinterpret_cast<uint2 *>(rec + qsb + (WT == WT_Q5_1 ? 64 : 0))[g] = make_uint2(d16(b0, r0) | (d16(b1, r1) << 16), m16(b0, r0) | (m16(b1, r1) << 16));
+        } else if (WT == WT_Q5_0) {
             auto h32 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[2] | ((uint32_t) blk[3] << 8) | ((uint32_t) blk[4] << 16) | ((uint32_t) blk[5] << 24)) : 0u; };
             reinterpret_cast<uint2 *>(rec + qsb)[g] = make_uint2(h32(b0, r0), h32(b1, r1));
             reinterpret_cast<uint32_t *>(rec + qsb + 64)[g] = d16(b0, r0) | (d16(b1, r1) << 16);
@@ -192,6 +204,8 @@ bool repack_tile_major(int wtype, const uint8_t * src, const QMat & dst, int row
         case WT_F16:  k_repack_tm<WT_F16><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
         case WT_Q4_0: k_repack_tm<WT_Q4_0><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
         case WT_Q5_0: k_repack_tm<WT_Q5_0><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
+        case WT_Q4_1: k_repack_tm<WT_Q4_1><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
+        case WT_Q5_1: k_repack_tm<WT_Q5_1><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
         case WT_Q8_0: k_repack_tm<WT_Q8_0><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
         default: set_error("repack_tile_major: bad type %d", wtype); return false;
     }
@@ -416,6 +430,16 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
         return __half2float(__ushort_as_half((unsigned short) ((i & 1) ? (w >> 16) : (w & 0xffffu))));
     }
     const int qsb = (W.type == WT_Q8_0) ? 512 : 256;
+    if (wt_has_min(W.type)) {                                    // dequantize_row_q4_1 / _q5_1: q * d + m
+        const uint2 dm = reinterpret_cast<const uint2 *>(rec + qsb + (W.type == WT_Q5_1 ? 64 : 0))[g];
+        const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dm.x >> 16) : (dm.x & 0xffffu))));
+        const float m = __half2float(__ushort_as_half((unsigned short) (up ? (dm.y >> 16) : (dm.y & 0xffffu))));
+        const int c = (i & 15) >> 2;
+        const uint32_t w = reinterpret_cast<const uint32_t *>(rec)[(g * 4 + c) * 2 + up];
+        int q = (int) ((w >> (8 * (i & 3) + 4 * (i >> 4))) & 0xFu);
+        if (W.type == WT_Q5_1) q |= (int) ((reinterpret_cast<const uint32_t *>(rec + 256)[g * 2 + up] >> i) & 1u) << 4;
+        return __fadd_rn(__fmul_rn((float) q, d), m);
+    }
     const uint32_t dd = reinterpret_cast<const uint32_t *>(rec + qsb + (W.type == WT_Q5_0 ? 64 : 0))[g];
     const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dd >> 16) : (dd & 0xffffu))));
     if (W.type == WT_Q8_0) {
@@ -441,6 +465,12 @@ __device__ __forceinline__ float dequant_elem(const QMat & W, int64_t row, int e
                         const uint8_t q = W.qs[b * 16 + (i & 15)]; const uint32_t h = (W.qh[b] >> i) & 1u;
                         const int v = (int) ((i < 16 ? (q & 0xF) : (q >> 4)) | (h << 4)) - 16;
                         return (float) v * __half2float(W.d[b]); }
+        case WT_Q4_1: case WT_Q5_1: {
+                        const int64_t b = row * (K >> 5) + (e >> 5); const int i = e & 31;
+                        const uint8_t q = W.qs[b * 16 + (i & 15)];
+                        int v = i < 16 ? (q & 0xF) : (q >> 4);
+                        if (W.type == WT_Q5_1) v |= (int) ((W.qh[b] >> i) & 1u) << 4;
+                        return __fadd_rn(__fmul_rn((float) v, __half2float(W.d[b])), __half2float(W.m[b])); }
         case WT_Q8_0: { const int64_t b = row * (K >> 5) + (e >> 5);
                         return (float) reinterpret_cast<const int8_t *>(W.qs)[b * 32 + (e & 31)] * __half2float(W.d[b]); }
         case WT_Q4_K: case WT_Q5_K: {
@@ -593,7 +623,12 @@ k_gemv(const GemvK a) {
             }
             uint4 * dst = reinterpret_cast<uint4 *>(tp + b * 32);
             dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]); dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            reinterpret_cast<float *>(tp + K)[b] = __half2float(__float2half_rn(d));
+            if (wt_has_min(WT)) {                                // Q8_1: {f16 d, f16 s = d * sum(q)} (quantize_row_q8_1, unrounded d)
+                int sum = 0;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) sum = __dp4a((int) pk[i], 0x01010101, sum);
+                reinterpret_cast<__half2 *>(tp + K)[b] = __halves2half2(__float2half_rn(d), __float2half_rn(d * (float) sum));
+            } else reinterpret_cast<float *>(tp + K)[b] = __half2float(__float2half_rn(d));
         }
     }
     __syncthreads();
@@ -658,6 +693,7 @@ k_gemv(const GemvK a) {
             for (int c = lane; c < K / 8; c += 32) {           // chunk = quarter block
                 const int b = c >> 2, qd = c & 3;
                 const float dw = __half2float(a.W.d[rb + b]);
+                const float mw = wt_has_min(WT) ? __half2float(a.W.m[rb + b]) : 0.0f;
                 int vl, vh;
                 if (WT == WT_Q8_0) {
                     const uint2 w = __ldg(reinterpret_cast<const uint2 *>(a.W.qs + (rb + b) * 32) + qd);
@@ -665,10 +701,13 @@ k_gemv(const GemvK a) {
                 } else {
                     const uint32_t w = __ldg(reinterpret_cast<const uint32_t *>(a.W.qs + (rb + b) * 16) + qd);
                     uint32_t lo = w & 0x0F0F0F0Fu, hi = (w >> 4) & 0x0F0F0F0Fu;
-                    if (WT == WT_Q5_0) {
+                    if (wt_has_qh(WT)) {
                         const uint32_t qh = __ldg(a.W.qh + rb + b);
                         lo |= spread4_to_bit4(qh >> (4 * qd));
                         hi |= spread4_to_bit4(qh >> (16 + 4 * qd));
+                    }
+                    if (wt_has_min(WT)) { vl = (int) lo; vh = (int) hi; }
+                    else if (WT == WT_Q5_0) {
                         vl = (int) __vsub4(lo, 0x10101010u); vh = (int) __vsub4(hi, 0x10101010u);
                     } else {
                         vl = (int) __vsub4(lo, 0x08080808u); vh = (int) __vsub4(hi, 0x08080808u);
@@ -684,6 +723,11 @@ k_gemv(const GemvK a) {
                         if (WT == WT_Q8_0) { xa = xq[b * 8 + 2 * qd]; xb = xq[b * 8 + 2 * qd + 1]; }
                         else               { xa = xq[b * 8 + qd];     xb = xq[b * 8 + 4 + qd]; }
                         const int sumi = __dp4a(vl, xa, __dp4a(vh, xb, 0));
+                        if (wt_has_min(WT)) {                    // ggml_vec_dot_q4_1_q8_1: (d_w d_x) sumi + m_w s_x, the m term once per block
+                            const __half2 ds = reinterpret_cast<const __half2 *>(tp + K)[b];
+                            acc[t] = fmaf(dw * __low2float(ds), (float) sumi, acc[t]);
+                            if (qd == 0) acc[t] = fmaf(mw, __high2float(ds), acc[t]);
+                        } else
                         acc[t] = fmaf(dw * dx, (float) sumi, acc[t]);
                     }
                 }
@@ -746,6 +790,8 @@ void gemv(const GemvArgs & a, cudaStream_t st) {
         case WT_F16:  gemv_nt<WT_F16>(k, st);  break;
         case WT_Q4_0: gemv_nt<WT_Q4_0>(k, st); break;
         case WT_Q5_0: gemv_nt<WT_Q5_0>(k, st); break;
+        case WT_Q4_1: gemv_nt<WT_Q4_1>(k, st); break;
+        case WT_Q5_1: gemv_nt<WT_Q5_1>(k, st); break;
         case WT_Q8_0: gemv_nt<WT_Q8_0>(k, st); break;
         case WT_Q4_K: gemv_nt<WT_Q4_K>(k, st); break;
         case WT_Q5_K: gemv_nt<WT_Q5_K>(k, st); break;
@@ -761,7 +807,7 @@ void gemv(const GemvArgs & a, cudaStream_t st) {
 //  vec_dot_q*_q8_0 (ggml-cpu/quants.c:365-406) and the dp4a kernel above; only the f32 summation order differs.
 //  One CTA = 32 output rows (two m16 tiles); its 8 warps split K and reduce through shared memory.
 // =====================================================================================================================
-template <int MODE>   // 0: Q8_0 blocks  1: Q8_K super-blocks  2: f16
+template <int MODE>   // 0: Q8_0 blocks  1: Q8_K super-blocks  2: f16  3: Q8_1 blocks
 __global__ void __launch_bounds__(256)
 k_act_quant(const float * __restrict__ x, int K, const float * __restrict__ ln_w, const float * __restrict__ ln_b, float eps,
             uint8_t * __restrict__ out, size_t tok_stride) {
@@ -818,14 +864,20 @@ k_act_quant(const float * __restrict__ x, int K, const float * __restrict__ ln_w
             if (lane == 0) xd[sb] = 1.0f / iscale;
         }
     } else {
-        // quantize_row_q8_0, AVX2 form (ggml-cpu/arch/x86/quants.c): warp per block, lane per element (coalesced)
+        // quantize_row_q8_0 / _q8_1, AVX2 form (ggml-cpu/arch/x86/quants.c): warp per block, lane per element (coalesced)
         for (int b = warp; b < K / 32; b += 8) {
             const float v = xval(b * 32 + lane);
             const float amax = warp_max(fabsf(v));
             const float d  = amax / 127.0f;
             const float id = (amax != 0.0f) ? 127.0f / amax : 0.0f;
-            reinterpret_cast<int8_t *>(tp)[b * 32 + lane] = (int8_t) __float2int_rn(v * id);
-            if (lane == 0) reinterpret_cast<float *>(tp + K)[b] = __half2float(__float2half_rn(d));
+            const int q = __float2int_rn(v * id);
+            reinterpret_cast<int8_t *>(tp)[b * 32 + lane] = (int8_t) q;
+            if (MODE == 3) {                                     // quantize_row_q8_1: {f16 d, f16 (d * sum q)}, d unrounded
+                int sum = q;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+                if (lane == 0) reinterpret_cast<__half2 *>(tp + K)[b] = __halves2half2(__float2half_rn(d), __float2half_rn(d * (float) sum));
+            } else if (lane == 0) reinterpret_cast<float *>(tp + K)[b] = __half2float(__float2half_rn(d));
         }
     }
 }
@@ -926,24 +978,28 @@ k_gemv_mma(const Gemv2K a) {
 #pragma unroll 5
         for (int b = warp; b < nblk; b += 8) {
             const uint32_t b0 = tok_ok ? xg[b * 8 + c] : 0u, b1 = tok_ok ? xg[b * 8 + 4 + c] : 0u;
-            const float dx0 = dx0p[b], dx1 = dx1p[b];
+            float dx0 = dx0p[b], dx1 = dx1p[b], sx0 = 0.0f, sx1 = 0.0f;
+            if (wt_has_min(WT)) {                                // Q8_1 rows: {f16 d, f16 s} in place of the f32 scale
+                const __half2 p0 = reinterpret_cast<const __half2 *>(dx0p)[b], p1 = reinterpret_cast<const __half2 *>(dx1p)[b];
+                dx0 = __low2float(p0); sx0 = __high2float(p0); dx1 = __low2float(p1); sx1 = __high2float(p1);
+            }
 #pragma unroll
             for (int mt = 0; mt < MT; ++mt) {
-                uint32_t af[4]; float dw[2];
+                uint32_t af[4]; float dw[2], mw[2] = { 0.0f, 0.0f };
 #pragma unroll
                 for (int r = 0; r < 2; ++r) {
                     const int64_t bi = (int64_t) rows[2*mt + r] * nblk + b;
                     const uint32_t * q32 = reinterpret_cast<const uint32_t *>(a.W.qs) + bi * QW;
                     dw[r] = __half2float(a.W.d[bi]);
+                    if (wt_has_min(WT)) mw[r] = __half2float(a.W.m[bi]);
                     if (WT == WT_Q8_0) { af[r] = __ldg(q32 + c); af[2 + r] = __ldg(q32 + 4 + c); }
                     else {
                         const uint32_t w = __ldg(q32 + c);
                         uint32_t lo = w & 0x0F0F0F0Fu, hi = (w >> 4) & 0x0F0F0F0Fu;
-                        if (WT == WT_Q5_0) {
-                            const uint32_t qh = __ldg(a.W.qh + bi);
-                            lo |= spread4_to_bit4(qh >> (4 * c)); hi |= spread4_to_bit4(qh >> (16 + 4 * c));
-                            af[r] = __vsub4(lo, 0x10101010u); af[2 + r] = __vsub4(hi, 0x10101010u);
-                        } else { af[r] = __vsub4(lo, 0x08080808u); af[2 + r] = __vsub4(hi, 0x08080808u); }
+                        if (wt_has_qh(WT)) { const uint32_t qh = __ldg(a.W.qh + bi); lo |= spread4_to_bit4(qh >> (4 * c)); hi |= spread4_to_bit4(qh >> (16 + 4 * c)); }
+                        if (wt_has_min(WT)) { af[r] = lo; af[2 + r] = hi; }
+                        else if (WT == WT_Q5_0) { af[r] = __vsub4(lo, 0x10101010u); af[2 + r] = __vsub4(hi, 0x10101010u); }
+                        else { af[r] = __vsub4(lo, 0x08080808u); af[2 + r] = __vsub4(hi, 0x08080808u); }
                     }
                 }
                 int dd[4]; mma_s8_16832(dd, af, b0, b1);
@@ -951,6 +1007,10 @@ k_gemv_mma(const Gemv2K a) {
                 acc[mt][1] = fmaf(dw[0] * dx1, (float) dd[1], acc[mt][1]);
                 acc[mt][2] = fmaf(dw[1] * dx0, (float) dd[2], acc[mt][2]);
                 acc[mt][3] = fmaf(dw[1] * dx1, (float) dd[3], acc[mt][3]);
+                if (wt_has_min(WT)) {                            // the block minimum against the activation block's sum (Q8_1 s)
+                    acc[mt][0] = fmaf(mw[0], sx0, acc[mt][0]); acc[mt][1] = fmaf(mw[0], sx1, acc[mt][1]);
+                    acc[mt][2] = fmaf(mw[1], sx0, acc[mt][2]); acc[mt][3] = fmaf(mw[1], sx1, acc[mt][3]);
+                }
             }
         }
     }
@@ -994,6 +1054,7 @@ void gemv2(const GemvArgs & a, uint8_t * act_scratch, cudaStream_t st) {
         ProfScope prof(PC_OTHER, st, 0.0, 0.0);
         if (a.W.type == WT_F16)           k_act_quant<2><<<a.n_tok, 256, 0, st>>>(a.x, K, a.ln_w, a.ln_b, a.eps, act_scratch, ts);
         else if (wt_is_kquant(a.W.type))  k_act_quant<1><<<a.n_tok, 256, 0, st>>>(a.x, K, a.ln_w, a.ln_b, a.eps, act_scratch, ts);
+        else if (wt_has_min(a.W.type))    k_act_quant<3><<<a.n_tok, 256, 0, st>>>(a.x, K, a.ln_w, a.ln_b, a.eps, act_scratch, ts);
         else                              k_act_quant<0><<<a.n_tok, 256, 0, st>>>(a.x, K, a.ln_w, a.ln_b, a.eps, act_scratch, ts);
         count_launch();
     }
@@ -1008,6 +1069,8 @@ void gemv2(const GemvArgs & a, uint8_t * act_scratch, cudaStream_t st) {
         case WT_F16:  WB_GEMV2(WT_F16);  break;
         case WT_Q4_0: WB_GEMV2(WT_Q4_0); break;
         case WT_Q5_0: WB_GEMV2(WT_Q5_0); break;
+        case WT_Q4_1: WB_GEMV2(WT_Q4_1); break;
+        case WT_Q5_1: WB_GEMV2(WT_Q5_1); break;
         case WT_Q8_0: WB_GEMV2(WT_Q8_0); break;
         case WT_Q4_K: WB_GEMV2(WT_Q4_K); break;
         case WT_Q5_K: WB_GEMV2(WT_Q5_K); break;

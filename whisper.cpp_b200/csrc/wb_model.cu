@@ -64,7 +64,8 @@ bool alloc_qmat(Model & m, int t, int N, int K, QMat & q, bool tile_major = fals
         const size_t nblk = (size_t) N * (K / 32);
         q.qs = (const uint8_t *) dalloc(m, nblk * wt_qs_bytes(t));
         q.d  = (const __half *)  dalloc(m, nblk * 2);
-        if (t == WT_Q5_0) { q.qh = (const uint32_t *) dalloc(m, nblk * 4); if (!q.qh) return false; }
+        if (wt_has_qh(t)) { q.qh = (const uint32_t *) dalloc(m, nblk * 4); if (!q.qh) return false; }
+        if (wt_has_min(t)) { q.m = (const __half *) dalloc(m, nblk * 2); if (!q.m) return false; }
         return q.qs && q.d;
     }
     if (wt_is_kquant(t)) {
@@ -72,7 +73,7 @@ bool alloc_qmat(Model & m, int t, int N, int K, QMat & q, bool tile_major = fals
         q.base = dalloc(m, (size_t) N * (K / 256) * (t == WT_Q4_K ? 144 : 176));
         return q.base != nullptr;
     }
-    set_error("model: unsupported weight type %d (supported: F32->F16, F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K)", t);
+    set_error("model: unsupported weight type %d (supported: F32->F16, F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q4_K, Q5_K)", t);
     return false;
 }
 
@@ -123,9 +124,9 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
     switch (hp.ftype) {  // ggml_ftype_to_ggml_type (ggml/src/ggml.c:1426-1463)
         case 0: m.wtype = WT_F32; break;  case 1: m.wtype = WT_F16; break; case 2: m.wtype = WT_Q4_0; break;
         case 7: m.wtype = WT_Q8_0; break; case 8: m.wtype = WT_Q5_0; break; case 12: m.wtype = WT_Q4_K; break;
-        case 13: m.wtype = WT_Q5_K; break;
+        case 13: m.wtype = WT_Q5_K; break; case 3: m.wtype = WT_Q4_1; break; case 9: m.wtype = WT_Q5_1; break;
         // formats without device kernels: expanded on the host at load time, kept in HBM as F16 (wb_dequant_host.h)
-        case 3: host_dq = HT_Q4_1; break; case 9: host_dq = HT_Q5_1; break; case 10: host_dq = HT_Q2_K; break;
+        case 10: host_dq = HT_Q2_K; break;
         case 11: host_dq = HT_Q3_K; break; case 14: host_dq = HT_Q6_K; break; case 24: host_dq = HT_BF16; break;
         default: set_error("invalid model (ftype %d is not supported by this engine)", hp.ftype); return false;
     }
@@ -365,7 +366,7 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
             } else if (wt_is_block32(q.type)) {
                 QMat sub = q;
                 const size_t boff = (size_t) D.row_off * (K / 32);
-                sub.qs = q.qs + boff * wt_qs_bytes(q.type); sub.d = q.d + boff; sub.qh = q.qh ? q.qh + boff : nullptr;
+                sub.qs = q.qs + boff * wt_qs_bytes(q.type); sub.d = q.d + boff; sub.qh = q.qh ? q.qh + boff : nullptr; sub.m = q.m ? q.m + boff : nullptr;
                 if (!repack_block32_into(q.type, dstage, sub, D.rows, K, 0)) return false;
             } else {
                 const size_t bpr = (size_t) (K / 256) * (q.type == WT_Q4_K ? 144 : 176);

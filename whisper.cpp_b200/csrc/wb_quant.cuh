@@ -1,6 +1,6 @@
 // wb_quant.cuh -- weight formats as they live in HBM, and the device-side decoders.
 //
-// File side (unchanged legacy ggml container): 32-value blocks block_q4_0 / block_q5_0 / block_q8_0
+// File side (unchanged legacy ggml container): 32-value blocks block_q4_0 / block_q4_1 / block_q5_0 / block_q5_1 / block_q8_0
 // (ggml/src/ggml-common.h:194-256) and 256-value super-blocks block_q4_K / block_q5_K
 // (ggml-common.h:327-356).  Bit-level meaning follows ggml/src/ggml-quants.c:459-567 (dequantize_row_q4_0,
 // _q5_0, _q8_0), :880-887 (get_scale_min_k4), :1529-1551 (q4_K), :1731-1756 (q5_K).
@@ -8,9 +8,10 @@
 // HBM side ("planar" layout, built once at load by wb_repack_*): the 18/22/34-byte file blocks are not
 // 16-byte aligned, so every 32-block matrix [N rows][K] is split into three dense arrays
 //     qs : [N][K/32][QS]   QS = 16 bytes (4/5-bit) or 32 bytes (8-bit)   -> one or two 128-bit loads per block
-//     qh : [N][K/32]       uint32, the fifth bits (Q5_0 only)
+//     qh : [N][K/32]       uint32, the fifth bits (Q5_0 / Q5_1)
 //     d  : [N][K/32]       f16 block scale
-// Total bytes are identical to the file (18 / 22 / 34 per 32 weights).  K-quant super-blocks are 144 / 176
+//     m  : [N][K/32]       f16 block minimum (Q4_1 / Q5_1: value = q * d + m, q unsigned)
+// Total bytes are identical to the file (18 / 20 / 22 / 24 / 34 per 32 weights).  K-quant super-blocks are 144 / 176
 // bytes = multiples of 16 and are kept verbatim (encoder side; the decoder matrices use the tile-major records below).
 #pragma once
 #include <cstdint>
@@ -19,7 +20,7 @@
 namespace wb {
 
 // numeric ids are ggml_type (ggml/include/ggml.h:390-405)
-enum WType : int { WT_F32 = 0, WT_F16 = 1, WT_Q4_0 = 2, WT_Q5_0 = 6, WT_Q8_0 = 8, WT_Q4_K = 12, WT_Q5_K = 13 };
+enum WType : int { WT_F32 = 0, WT_F16 = 1, WT_Q4_0 = 2, WT_Q4_1 = 3, WT_Q5_0 = 6, WT_Q5_1 = 7, WT_Q8_0 = 8, WT_Q4_K = 12, WT_Q5_K = 13 };
 
 struct QMat {            // one weight matrix resident in HBM
     int   type = WT_F16;
@@ -28,6 +29,7 @@ struct QMat {            // one weight matrix resident in HBM
     const uint8_t  * qs = nullptr;
     const uint32_t * qh = nullptr;
     const __half   * d  = nullptr;
+    const __half   * m  = nullptr;   // Q4_1 / Q5_1 planar: block minima
     int   layout = 0;    // 0: rows (F16) / planar (32-blocks) / verbatim (K-quants); 1: tile-major records at `base` (see below)
     const __half * f16 = nullptr;  // encoder-side matrices of quantised models: f16 expansion [N][K] made once at load (TMA operand of the
                                    // persistent GEMM; each value is the f16 rounding of the exact d * (q - off)); nullptr = expand per launch
@@ -38,6 +40,9 @@ struct QMat {            // one weight matrix resident in HBM
 // operands in the register order of the warp-level MMA (lane = 4*g + c reads rows g and g+8 of the tile):
 //   Q4_0 (288 B): u32 qs[32 lanes][2] = { word c of row g, word c of row g+8 }            | f16 d[8][2]  = { row g, row g+8 }
 //   Q5_0 (352 B): qs as Q4_0 (256 B) | u32 qh[8][2] = { row g, row g+8 } (64 B)            | f16 d[8][2]
+//   Q4_1 (320 B): qs as Q4_0, unsigned nibbles (256 B)                                     | u32 dm[8][2] = { d_g | d_g+8 << 16, m_g | m_g+8 << 16 }
+//   Q5_1 (384 B): qs as Q4_1 (256 B) | qh as Q5_0 (64 B)                                   | dm as Q4_1
+//   (one 8-byte load gives lane 4g + c the scales and minima of both its rows)
 //   Q8_0 (544 B): u32 qs[32 lanes][4] = { w c / row g, w c / row g+8, w 4+c / row g, w 4+c / row g+8 } | f16 d[8][2]
 //   F16  (512 B per 16 values): u32 a[32 lanes][4] = the m16n8k16 A fragment
 // so one warp fetches a record with three fully coalesced loads.  Same bytes per weight as the file; rows >= N are zero.
@@ -48,18 +53,21 @@ struct QMat {            // one weight matrix resident in HBM
 // = the file's 16 x 144 / 16 x 176 bytes.  The GEMV splits K per 32-value sub-block (record + 256 + j * 256 / 320); a lane reads 8 bytes
 // of the header: lane 4g + c gets bytes 8 (c & 1) .. +7 of row g + 8 (c >> 1), so a quad holds the 32 header bytes of its two rows.
 __host__ __device__ inline int wt_tm_rec_bytes(int t) {
-    return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 : 0;
+    return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q4_1 ? 320 : t == WT_Q5_1 ? 384 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 : 0;
 }
 __host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : (t == WT_Q4_K || t == WT_Q5_K) ? 256 : 32; }
 __host__ __device__ inline int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : 320; }      // K-quants: one 32-value sub-block record
 __host__ __device__ inline size_t wt_tm_bytes(int t, int N, int K) { return (size_t) ((N + 15) / 16) * (K / wt_tm_rec_k(t)) * wt_tm_rec_bytes(t); }
 
 __host__ __device__ inline int wt_qs_bytes(int t)    { return t == WT_Q8_0 ? 32 : 16; }
-__host__ __device__ inline bool wt_is_block32(int t) { return t == WT_Q4_0 || t == WT_Q5_0 || t == WT_Q8_0; }
+__host__ __device__ inline bool wt_is_block32(int t) { return t == WT_Q4_0 || t == WT_Q5_0 || t == WT_Q8_0 || t == WT_Q4_1 || t == WT_Q5_1; }
+__host__ __device__ inline bool wt_has_min(int t)    { return t == WT_Q4_1 || t == WT_Q5_1; }     // blocks with a minimum: Q8_1 activations
+__host__ __device__ inline bool wt_has_qh(int t)     { return t == WT_Q5_0 || t == WT_Q5_1; }
 __host__ __device__ inline bool wt_is_kquant(int t)  { return t == WT_Q4_K || t == WT_Q5_K; }
 // bytes per weight on disk and in HBM
 __host__ __device__ inline double wt_bpw(int t) {
     switch (t) { case WT_F32: return 4; case WT_F16: return 2; case WT_Q4_0: return 18.0/32; case WT_Q5_0: return 22.0/32;
+                 case WT_Q4_1: return 20.0/32; case WT_Q5_1: return 24.0/32;
                  case WT_Q8_0: return 34.0/32; case WT_Q4_K: return 144.0/256; case WT_Q5_K: return 176.0/256; }
     return 0;
 }
@@ -126,6 +134,43 @@ __device__ __forceinline__ void dequant_q8_0(const uint4 q0, const uint4 q1, con
     }
     out[0] = make_uint4(h[0], h[1], h[2], h[3]);   out[1] = make_uint4(h[4], h[5], h[6], h[7]);
     out[2] = make_uint4(h[8], h[9], h[10], h[11]); out[3] = make_uint4(h[12], h[13], h[14], h[15]);
+}
+
+// Q4_1 / Q5_1: 32 unsigned values (bytes of q: element order of dequant_q4_0 / _q5_0) -> y = q * d + m evaluated in f32 (each
+// product and sum rounded: dequantize_row_q4_1 / _q5_1 without contraction), then rounded once to f16
+__device__ __forceinline__ void dequant_q1_bytes(const uint32_t (&lo)[4], const uint32_t (&hi)[4], float d, float m, uint4 (&out)[4]) {
+    uint32_t h[16];
+#pragma unroll
+    for (int v = 0; v < 2; ++v)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t b = v ? hi[i] : lo[i];
+            float f[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) f[e] = __fadd_rn(__fmul_rn((float) ((b >> (8 * e)) & 0xFFu), d), m);
+            const __half2 a = __floats2half2_rn(f[0], f[1]), c = __floats2half2_rn(f[2], f[3]);
+            h[8 * v + 2 * i]     = *reinterpret_cast<const uint32_t *>(&a);
+            h[8 * v + 2 * i + 1] = *reinterpret_cast<const uint32_t *>(&c);
+        }
+    out[0] = make_uint4(h[0], h[1], h[2], h[3]);   out[1] = make_uint4(h[4], h[5], h[6], h[7]);
+    out[2] = make_uint4(h[8], h[9], h[10], h[11]); out[3] = make_uint4(h[12], h[13], h[14], h[15]);
+}
+__device__ __forceinline__ void dequant_q4_1(const uint4 qs, const __half d, const __half m, uint4 (&out)[4]) {
+    const uint32_t w[4] = { qs.x, qs.y, qs.z, qs.w };
+    uint32_t lo[4], hi[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { lo[i] = w[i] & 0x0F0F0F0Fu; hi[i] = (w[i] >> 4) & 0x0F0F0F0Fu; }
+    dequant_q1_bytes(lo, hi, __half2float(d), __half2float(m), out);
+}
+__device__ __forceinline__ void dequant_q5_1(const uint4 qs, const uint32_t qh, const __half d, const __half m, uint4 (&out)[4]) {
+    const uint32_t w[4] = { qs.x, qs.y, qs.z, qs.w };
+    uint32_t lo[4], hi[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        lo[i] = ( w[i]       & 0x0F0F0F0Fu) | spread4_to_bit4(qh >> (4*i));
+        hi[i] = ((w[i] >> 4) & 0x0F0F0F0Fu) | spread4_to_bit4(qh >> (16 + 4*i));
+    }
+    dequant_q1_bytes(lo, hi, __half2float(d), __half2float(m), out);
 }
 
 // 6-bit scale / min of sub-block j (0..7) from the 12 packed bytes (ggml-quants.c:880-887)

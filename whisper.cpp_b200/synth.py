@@ -7,8 +7,8 @@ reversed dims and no padding.  2-D weights are quantised like `whisper-quantize`
 the two positional embeddings; conv kernels stay F16, 1-D tensors F32; ftype in the header becomes 2000 + ftype.
 
 The block quantisers restate ggml's reference quantisers (ggml/src/ggml-quants.c: quantize_row_q4_0_ref :113-147,
-quantize_row_q5_0_ref :187-229, quantize_row_q8_0_ref :276-299); tests/test_synth_cpu.py checks them
-bit-for-bit against the compiled reference.  Host-side tooling only: no dependency on oracle/.
+quantize_row_q5_0_ref :187-229, quantize_row_q8_0_ref :276-299, quantize_row_q4_1_ref :150-185, quantize_row_q5_1_ref :231-274);
+tests/test_synth_cpu.py and tests/test_q8_1_cpu.py check them bit-for-bit against the compiled reference.  Host-side tooling only: no dependency on oracle/.
 """
 import struct
 import zlib
@@ -16,7 +16,8 @@ import zlib
 import numpy as np
 
 F32, F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K = 0, 1, 2, 6, 8, 12, 13
-Q4_1, Q5_1, Q2_K, Q3_K, Q6_K, BF16 = 3, 7, 10, 11, 14, 30              # no NumPy quantiser here: pass quantizer= (ggml's own, via the oracle build)
+Q4_1, Q5_1 = 3, 7
+Q2_K, Q3_K, Q6_K, BF16 = 10, 11, 14, 30              # no NumPy quantiser here: pass quantizer= (ggml's own, via the oracle build)
 FTYPE_OF = {F32: 0, F16: 1, Q4_0: 2, Q8_0: 7, Q5_0: 8, Q4_K: 12, Q5_K: 13, Q4_1: 3, Q5_1: 9, Q2_K: 10, Q3_K: 11, Q6_K: 14, BF16: 24}
 
 CONFIGS = {
@@ -32,6 +33,8 @@ CONFIGS = {
     "test-3l.en":     (51864, 1500, 384, 6, 2, 448, 384, 6, 3, 80),     # 3 text layers: timestamps stay on
     "test-2l-512.en": (51864, 1500, 512, 8, 2, 448, 512, 8, 2, 80),
     "test-2l-multi":  (51866, 1500, 256, 4, 2, 448, 256, 4, 2, 128),
+    "small.en":       (51864, 1500, 768, 12, 12, 448, 768, 12, 12, 80),
+    "test-2l-768.en": (51864, 1500, 768, 12, 2, 448, 768, 12, 2, 80),     # the small.en width at a depth the CPU reference finishes in seconds
 }
 
 
@@ -108,9 +111,34 @@ def quantize(wtype, w):
         out[:, 2:6] = qh.view(np.uint8).reshape(nb, 4)
         out[:, 6:] = ((q[:, :16] & 0xF) | ((q[:, 16:] & 0xF) << 4)).astype(np.uint8)
         return out.tobytes()
+    if wtype in (Q4_1, Q5_1):
+        return quantize_q1(wtype, x)
     if wtype == Q4_K:
         return quantize_q4_k_simple(w)
     raise ValueError(f"synth.quantize: type {wtype} needs an external quantiser (pass quantizer=...)")
+
+
+def quantize_q1(wtype, x):
+    """[nb][32] float32 -> block_q4_1 / block_q5_1 bytes (quantize_row_q4_1_ref / _q5_1_ref): d = (max - min) / 15 (31), m = min,
+    q = (x - min) * (1/d) + 0.5 truncated (Q4_1: capped at 15)"""
+    nb = x.shape[0]
+    mn = x.min(axis=1); mx = x.max(axis=1)
+    d = ((mx - mn) / np.float32(15.0 if wtype == Q4_1 else 31.0)).astype(np.float32)
+    idv = np.where(d != 0, np.float32(1.0) / np.where(d != 0, d, 1), 0).astype(np.float32)
+    t = ((x - mn[:, None]).astype(np.float32) * idv[:, None]).astype(np.float32) + np.float32(0.5)
+    q = t.astype(np.int32)
+    out = np.empty((nb, 20 if wtype == Q4_1 else 24), np.uint8)
+    out[:, 0:2] = d.astype(np.float16).view(np.uint8).reshape(nb, 2)
+    out[:, 2:4] = mn.astype(np.float16).view(np.uint8).reshape(nb, 2)
+    if wtype == Q4_1:
+        q = np.minimum(15, q).astype(np.uint8)
+        out[:, 4:] = q[:, :16] | (q[:, 16:] << 4)
+        return out.tobytes()
+    q = q.astype(np.uint32)
+    qh = (((q >> 4) & 1) << np.arange(32, dtype=np.uint32)[None, :]).sum(axis=1, dtype=np.uint64).astype(np.uint32)
+    out[:, 4:8] = qh.view(np.uint8).reshape(nb, 4)
+    out[:, 8:] = ((q[:, :16] & 0xF) | ((q[:, 16:] & 0xF) << 4)).astype(np.uint8)
+    return out.tobytes()
 
 
 def quantize_q4_k_simple(w):
@@ -214,7 +242,7 @@ def write_model(path, config="test-2l.en", wtype=F16, seed=0, sigma=0.02, vocab_
     n_vocab, n_actx, d, n_ah, La, n_tctx, dt, n_th, Lt, n_mels = cfg
     q = quantizer or quantize
     ftype = FTYPE_OF[wtype] + (2000 if wtype not in (F32, F16) else 0)
-    blk = {Q4_0: (32, 18), Q5_0: (32, 22), Q8_0: (32, 34), Q4_K: (256, 144), Q5_K: (256, 176)}.get(wtype)
+    blk = {Q4_0: (32, 18), Q5_0: (32, 22), Q8_0: (32, 34), Q4_1: (32, 20), Q5_1: (32, 24), Q4_K: (256, 144), Q5_K: (256, 176)}.get(wtype)
     pool = None
     if fast_pool:
         prng = np.random.default_rng(seed ^ 0x5EED)
@@ -291,7 +319,7 @@ def cached_model(config, wtype, seed=0, fast_pool=False, tag=None):
     """a synthetic model in the temp directory, written once per box (the multi-GB ones take a while); returns its path"""
     import os
     import tempfile
-    names = {F16: "f16", Q4_0: "q4_0", Q5_0: "q5_0", Q8_0: "q8_0", Q4_K: "q4_k"}
+    names = {F16: "f16", Q4_0: "q4_0", Q5_0: "q5_0", Q8_0: "q8_0", Q4_K: "q4_k", Q4_1: "q4_1", Q5_1: "q5_1"}
     path = os.path.join(tempfile.gettempdir(), "wb200-%s-%s%s.bin" % (config, names[wtype], ("-" + tag) if tag else ""))
     if not os.path.exists(path):
         tmp = path + ".tmp.%d" % os.getpid()
