@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Q4_K decoding: the persistent decode kernel (64 rows per pass) against the kernel-per-op chain (8 rows per pass), in one process.
+"""K-quant decoding (Q4_K by default, --wtype q3_k): the persistent decode kernel (64 rows per pass) against the kernel-per-op chain (8 rows per pass), in one process.
 
-Model: synth.cached_model("large-v3", Q4_K, seed=0, fast_pool=True), the model of `bench.py --config 3`.
+Model: synth.cached_model("large-v3", Q4_K, seed=0, fast_pool=True), the model of `bench.py --config 3` (or the Q3_K one).
 Arms (the decoder layout is fixed when a context is created, so the switch is set before each context):
   new   -- default (tile-major K-quant records, persistent kernel)
   chain -- WB200_MEGAKERNEL=0
@@ -101,13 +101,14 @@ def main():
     ap.add_argument("--minutes", type=float, default=3.0, help="audio of workload b")
     ap.add_argument("--workloads", default="ab")
     ap.add_argument("--f16", action="store_true", help="add the WB200_KQUANT_AS_F16=1 arm")
+    ap.add_argument("--wtype", choices=("q4_k", "q3_k"), default="q4_k", help="block format of the synthetic large-v3 model")
     args = ap.parse_args()
     pkg = load_pkg(); synth = pkg.synth
     if not os.environ.get("WB200_VERBOSE"):                     # the library's INFO lines off stdout (whisper_log_set)
         lib = C.CDLL(pkg.LIB_PATH)
         lib.whisper_log_set.argtypes = [LOG_CB, C.c_void_p]
         lib.whisper_log_set(QUIET, None)
-    model = synth.cached_model("large-v3", synth.Q4_K, seed=0, fast_pool=True)
+    model = synth.cached_model("large-v3", {"q4_k": synth.Q4_K, "q3_k": synth.Q3_K}[args.wtype], seed=0, fast_pool=True)
     arms = ["new", "chain"] + (["f16"] if args.f16 else [])
     gpu = card()
     inputs = {"a": (np.concatenate([synth.synth_audio(seed=i, seconds=30.0) for i in range(64)]), 64),

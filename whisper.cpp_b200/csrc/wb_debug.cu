@@ -225,17 +225,18 @@ int wb200_dbg_tm_dequant(int wtype, int N, int K, const void * w_file, float * o
     return 0;
 }
 
-// W [N][K] in FILE layout -> planar 32-blocks on the device (the encoder's and the kernel chain's layout) -> every element read back through
-// the token-embedding reader: out f32 [N][K]
+// W [N][K] in FILE layout -> planar 32-blocks (K-quants: the verbatim super-blocks) on the device (the encoder's and the kernel chain's
+// layout) -> every element read back through the token-embedding reader: out f32 [N][K]
 __attribute__((visibility("default")))
 int wb200_dbg_planar_dequant(int wtype, int N, int K, const void * w_file, float * out) {
-    if (!wt_is_block32(wtype) || K % 32) { set_error("wb200_dbg_planar_dequant: no planar layout for type %d, K=%d", wtype, K); return -5; }
+    if (!(wt_is_block32(wtype) || wt_is_kquant(wtype)) || K % wt_tm_rec_k(wtype)) { set_error("wb200_dbg_planar_dequant: no planar layout for type %d, K=%d", wtype, K); return -5; }
     DevBuf<uint8_t> wraw, planar; DevBuf<float> dout;
     const size_t wbytes = (size_t) ((double) N * K * wt_bpw(wtype) + 0.5);
     if (!wraw.alloc(wbytes) || !planar.alloc(wbytes + 64) || !dout.alloc((size_t) N * K)) return -1;
     WB_CUDA_OKV(cudaMemcpy(wraw.p, w_file, wbytes, cudaMemcpyHostToDevice), -2);
     QMat W;
-    if (!repack_block32(wtype, wraw.p, planar.p, N, K, &W, 0)) return -4;
+    if (wt_is_kquant(wtype)) { W.type = wtype; W.N = N; W.K = K; W.base = wraw.p; }
+    else if (!repack_block32(wtype, wraw.p, planar.p, N, K, &W, 0)) return -4;
     dequant_rows_f32(W, dout.p, 0);
     WB_CUDA_OKV(cudaMemcpy(out, dout.p, (size_t) N * K * 4, cudaMemcpyDeviceToHost), -2);
     return 0;

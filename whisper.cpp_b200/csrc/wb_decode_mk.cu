@@ -145,7 +145,8 @@ __device__ __noinline__ void mk_grid_sync(const MkArgs & a, const MkView v, unsi
 // by one K/8-byte record per row (the size of the Q8_0 scales, so the staging is the same): f32 d[K/256] | int16 sum[K/32] of each
 // 32 quantised values (the dmin term).  A 256-value super-block needs its signed value of largest magnitude: producers that see
 // less than a super-block (attention heads, FC1 tiles) write f32 rows, and a quantise phase (mk_q8k_rows) follows them.
-constexpr bool mk_kq(int WT) { return WT == WT_Q4_K || WT == WT_Q5_K; }
+// Q3_K uses the same rows without the sums: signed weights, one integer scale per 16 values, no minimum.
+constexpr bool mk_kq(int WT) { return WT == WT_Q4_K || WT == WT_Q5_K || WT == WT_Q3_K; }
 
 // Q4_1 / Q5_1 weights: rows are Q8_1 (quantize_row_q8_1, AVX2 form ggml-cpu/arch/x86/quants.c): the int8 values of Q8_0 (with the IEEE
 // quotients 127/amax and amax/127 the reference uses), and in place of each f32 block scale the pair {f16 d, f16 s = d * sum(q)} (s from
@@ -373,9 +374,9 @@ __device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_all;
 // 2.4 us for three slots): an iteration with four slots makes two calls of two slots, same partials, no spills.
 template <int WT, int NV, int TU, int KS, int UB>
 __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * wbase, int tile0, int tstep, int nrec, int nb, int SW, int nt, int NH, bool & staged, uint32_t stage_parity, int fb, int j0) {
-    constexpr bool KQ = mk_kq(WT), Q1 = mk_q1(WT);
+    constexpr bool KQ = mk_kq(WT), Q3K = (WT == WT_Q3_K), Q1 = mk_q1(WT);
     constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
-                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : 512))));   // K-quants: bytes per 32 values
+                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : (WT == WT_Q3_K ? 228 : 512)))));   // K-quants: bytes per 32 values
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RLD = 17;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3, ks = warp & (KS - 1);
@@ -392,6 +393,14 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                 const uint8_t * tb = wbase + (size_t) ((tile0 + ((j0 + j) / TU) * tstep) * TU + (j0 + j) % TU) * nrec * REC;
 #pragma unroll
                 for (int u = 0; u < UB; ++u) {
+                    if (Q3K) {                                   // Q3_K sub-block record + this lane's scale word and d word
+                        const int bb = min(kb + u * KS, nrec - 1);
+                        const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 288 + (bb & 7) * wt_tm_sub_bytes(WT);
+                        wq[j][u].x = __ldg(reinterpret_cast<const uint32_t *>(rec) + lane);
+                        wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + 128) + g);
+                        wk[j][u] = make_uint2(__ldg(reinterpret_cast<const uint32_t *>(sbp) + (bb & 7) * 8 + g), __ldg(reinterpret_cast<const uint32_t *>(sbp + 256) + g));
+                        continue;
+                    }
                     if (KQ) {                                    // sub-block record of super-block sb (wb_quant.cuh) + this lane's 8 header bytes
                         const int bb = min(kb + u * KS, nrec - 1);
                         const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
@@ -424,8 +433,10 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                     if (KQ) {                                    // Q8_K: d of the super-block, sum of the sub-block (mk_store_q comment)
                         const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
                         dx[h][0] = SM_XD[r0 * nb + (b >> 3)]; dx[h][1] = SM_XD[r1 * nb + (b >> 3)];
-                        sx[h][0] = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
-                        sx[h][1] = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+                        if (!Q3K) {
+                            sx[h][0] = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
+                            sx[h][1] = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+                        }
                     } else if (Q1) {                             // Q8_1: {d, s} of the block
                         const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c, nt - 1) * nb + b];
                         const __half2 p1 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
@@ -434,6 +445,23 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
                 }
 #pragma unroll
                 for (int j = 0; j < NV; ++j) {
+                    if (Q3K) {                                   // signed 3-bit weights; acc += (d_w d_x) (sc_lo sumi_lo + sc_hi sumi_hi)
+                        uint32_t af[4];
+                        q3k_tm_af(wq[j][u].x, wh[j][u], c, af);
+                        const float dw0 = __half2float(__ushort_as_half((unsigned short) (wk[j][u].y & 0xffffu)));
+                        const float dw1 = __half2float(__ushort_as_half((unsigned short) (wk[j][u].y >> 16)));
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            if (h < NH) {
+                                int si[4]; q3k_sumi(af, bf[h][0], bf[h][1], wk[j][u].x, si);
+                                acc[j][h][0] = fmaf(dw0 * dx[h][0], (float) si[0], acc[j][h][0]);
+                                acc[j][h][1] = fmaf(dw0 * dx[h][1], (float) si[1], acc[j][h][1]);
+                                acc[j][h][2] = fmaf(dw1 * dx[h][0], (float) si[2], acc[j][h][2]);
+                                acc[j][h][3] = fmaf(dw1 * dx[h][1], (float) si[3], acc[j][h][3]);
+                            }
+                        }
+                        continue;
+                    }
                     if (KQ) {                                    // unsigned 4 / 5-bit weights; acc += d_x * (d sc_j * sumi - dmin m_j * sumx) as the chain
                         uint32_t af[4];
                         af[0] = wq[j][u].x & 0x0F0F0F0Fu; af[2] = (wq[j][u].x >> 4) & 0x0F0F0F0Fu;
@@ -658,9 +686,9 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
 // is one accumulator over the blocks in ascending order: independent of the batch.
 template <int WT>
 __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, float * out) {
-    constexpr bool KQ = mk_kq(WT), Q1 = mk_q1(WT);
+    constexpr bool KQ = mk_kq(WT), Q3K = (WT == WT_Q3_K), Q1 = mk_q1(WT);
     constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
-                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : 512))));
+                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : (WT == WT_Q3_K ? 228 : 512)))));
     constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
     constexpr int RK = (WT == WT_F16) ? 16 : 32;
     constexpr int UB = 8;
@@ -699,6 +727,14 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
             uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB]; uint2 wk[UB]; uint2 wm[UB];
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
+                if (Q3K) {
+                    const int bb = min(kb + u, nrec - 1);
+                    const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 288 + (bb & 7) * wt_tm_sub_bytes(WT);
+                    wq[u].x = __ldg(reinterpret_cast<const uint32_t *>(rec) + lane);
+                    wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + 128) + g);
+                    wk[u] = make_uint2(__ldg(reinterpret_cast<const uint32_t *>(sbp) + (bb & 7) * 8 + g), __ldg(reinterpret_cast<const uint32_t *>(sbp + 256) + g));
+                    continue;
+                }
                 if (KQ) {
                     const int bb = min(kb + u, nrec - 1);
                     const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
@@ -718,7 +754,26 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
                 const int b = kb + u;
-                if (KQ && b < nrec) {
+                if (Q3K && b < nrec) {
+                    uint32_t af[4];
+                    q3k_tm_af(wq[u].x, wh[u], c, af);
+                    const float dw0 = __half2float(__ushort_as_half((unsigned short) (wk[u].y & 0xffffu)));
+                    const float dw1 = __half2float(__ushort_as_half((unsigned short) (wk[u].y >> 16)));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (h < NH) {
+                            const bool ok = h * 8 + g < nt;
+                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
+                            const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
+                            const float dx0 = SM_XD[r0 * nb + (b >> 3)], dx1 = SM_XD[r1 * nb + (b >> 3)];
+                            int si[4]; q3k_sumi(af, b0, b1, wk[u].x, si);
+                            acc[h][0] = fmaf(dw0 * dx0, (float) si[0], acc[h][0]);
+                            acc[h][1] = fmaf(dw0 * dx1, (float) si[1], acc[h][1]);
+                            acc[h][2] = fmaf(dw1 * dx0, (float) si[2], acc[h][2]);
+                            acc[h][3] = fmaf(dw1 * dx1, (float) si[3], acc[h][3]);
+                        }
+                    }
+                } else if (KQ && b < nrec) {
                     uint32_t af[4];
                     af[0] = wq[u].x & 0x0F0F0F0Fu; af[2] = (wq[u].x >> 4) & 0x0F0F0F0Fu;
                     af[1] = wq[u].y & 0x0F0F0F0Fu; af[3] = (wq[u].y >> 4) & 0x0F0F0F0Fu;
@@ -1223,6 +1278,7 @@ bool mk_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st) {
         case WT_Q8_0: return WB_MK(WT_Q8_0);
         case WT_Q4_K: return WB_MK(WT_Q4_K);
         case WT_Q5_K: return WB_MK(WT_Q5_K);
+        case WT_Q3_K: return WB_MK(WT_Q3_K);
         default: set_error("decode megakernel: unsupported weight type %d", wtype); return false;
     }
 #undef WB_MK

@@ -366,6 +366,11 @@ gemm_kernel(const GemmKParams p, const __grid_constant__ CUtensorMap tmA, const 
                             uint4 q[4];
                             dequant_kq_sub<WT == WT_Q5_K>(rowp + (int64_t) (k >> 8) * BLK, (k & 255) >> 5, q);
                             oh[0] = q[0]; oh[1] = q[1]; oh[2] = q[2]; oh[3] = q[3];
+                        } else if (WT == WT_Q3_K) {
+                            const uint8_t * rowp = reinterpret_cast<const uint8_t *>(p.a_base) + (int64_t) m * (p.K >> 8) * 110;
+                            uint4 q[4];
+                            dequant_q3k_sub(rowp + (int64_t) (k >> 8) * 110, (k & 255) >> 5, q);
+                            oh[0] = q[0]; oh[1] = q[1]; oh[2] = q[2]; oh[3] = q[3];
                         } else {
                             RawBlk rb; uint4 q[4];
                             raw_load<WT>(p, m, k, rb, true);
@@ -440,6 +445,9 @@ k_dequant_f16(const void * base, const uint8_t * qs, const uint32_t * qh, const 
         const int64_t row = bi / nblk, kb = bi - row * nblk;
         const uint8_t * sb = reinterpret_cast<const uint8_t *>(base) + ((row0 + row) * (K >> 8) + (kb >> 3)) * BLK;
         dequant_kq_sub<WT == WT_Q5_K>(sb, (int) (kb & 7), o);
+    } else if (WT == WT_Q3_K) {
+        const int64_t row = bi / nblk, kb = bi - row * nblk;
+        dequant_q3k_sub(reinterpret_cast<const uint8_t *>(base) + ((row0 + row) * (K >> 8) + (kb >> 3)) * 110, (int) (kb & 7), o);
     } else {
         const int64_t g = row0 * nblk + bi;
         if (WT == WT_Q4_0)      dequant_q4_0(__ldg(reinterpret_cast<const uint4 *>(qs) + g), dd[g], o);
@@ -549,6 +557,7 @@ cudaError_t dequant_to_f16(const QMat & W, int64_t rows, __half * out, cudaStrea
         case WT_Q8_0: k_dequant_f16<WT_Q8_0><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
         case WT_Q4_K: k_dequant_f16<WT_Q4_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
         case WT_Q5_K: k_dequant_f16<WT_Q5_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
+        case WT_Q3_K: k_dequant_f16<WT_Q3_K><<<grid, 256, 0, st>>>(W.base, W.qs, W.qh, W.d, W.m, 0, n_blocks, W.K, out); break;
         default: return cudaErrorInvalidValue;
     }
     count_launch();
@@ -587,6 +596,7 @@ cudaError_t gemm_launch(const GemmDesc & g, cudaStream_t st) {
         case WT_Q8_0: return launch_ek<WT_Q8_0>(g, kp, false, st);
         case WT_Q4_K: return launch_ek<WT_Q4_K>(g, kp, false, st);
         case WT_Q5_K: return launch_ek<WT_Q5_K>(g, kp, false, st);
+        case WT_Q3_K: return launch_ek<WT_Q3_K>(g, kp, false, st);
     }
     return cudaErrorInvalidValue;
 }

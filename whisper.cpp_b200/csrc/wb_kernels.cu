@@ -183,6 +183,52 @@ __global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __res
     }
 }
 
+// Q3_K tile-major records (wb_quant.cuh): one thread per (tile, 32-value sub-block, lane); the lanes of sub-block 0 also write the
+// header (scale words lane and lane + 32, d words of lanes 0 .. 7)
+__global__ void k_repack_tm_q3k(const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int rows, int K, int64_t n_threads) {
+    constexpr int BLK = 110;
+    const int REC = wt_tm_rec_bytes(WT_Q3_K), SUB = wt_tm_sub_bytes(WT_Q3_K), nsub = K / 32, nsb = K / 256;
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_threads) return;
+    const int lane = (int) (i & 31), g = lane >> 2, c = lane & 3;
+    const int64_t rb = i >> 5;
+    const int b = (int) (rb % nsub), sb = b >> 3, j = b & 7;
+    const int64_t tile = rb / nsub;
+    uint8_t * sbp = dst + (tile * nsb + sb) * REC;
+    uint8_t * rec = sbp + 288 + j * SUB;
+    const int64_t r0 = tile * 16 + g, r1 = r0 + 8;
+    auto blk = [&](int64_t r) { return src + (r * nsb + sb) * BLK; };
+    // stored values q + 4 of values 32 j + v .. + 3 of row r; rows >= N: 0 (their scales are 0)
+    auto uval4 = [&](int64_t r, int v) -> uint32_t { return r < rows ? __vadd4(q3k_q4(blk(r), 32 * j + v), 0x04040404u) : 0u; };
+    // the lane's A registers: r = 0 / 1 rows g / g + 8 values 4c .., r = 2 / 3 values 16 + 4c ..
+    const uint32_t u[4] = { uval4(r0, 4 * c), uval4(r1, 4 * c), uval4(r0, 16 + 4 * c), uval4(r1, 16 + 4 * c) };
+    uint32_t lw = 0;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) lw |= (u[r] & 0x03030303u) << (2 * r);
+    reinterpret_cast<uint32_t *>(rec)[lane] = lw;
+    if (c == 0) {                                                // high bits of the 32 values of rows g, g + 8 (bit v = value v)
+        auto hbits = [&](int64_t r) -> uint32_t {
+            uint32_t h = 0;
+            for (int v = 0; v < 32; v += 4) h |= spread_bit2(uval4(r, v)) << v;
+            return h;
+        };
+        reinterpret_cast<uint2 *>(rec + 128)[g] = make_uint2(hbits(r0), hbits(r1));
+    }
+    if (j == 0) {                                                // header
+        auto sc = [&](int64_t r, int is) -> uint32_t { return r < rows ? (uint32_t) (q3k_scale(blk(r), is) & 0xff) : 0u; };
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const int w = lane + 32 * k, jj = w >> 3, gg = w & 7;
+            const int64_t ra = tile * 16 + gg, rb8 = ra + 8;
+            reinterpret_cast<uint32_t *>(sbp)[w] = sc(ra, 2 * jj) | (sc(ra, 2 * jj + 1) << 8) | (sc(rb8, 2 * jj) << 16) | (sc(rb8, 2 * jj + 1) << 24);
+        }
+        if (lane < 8) {
+            const int64_t ra = tile * 16 + lane, rb8 = ra + 8;
+            reinterpret_cast<uint32_t *>(sbp + 256)[lane] = (ra < rows ? q3k_dbits(blk(ra)) : 0u) | ((rb8 < rows ? q3k_dbits(blk(rb8)) : 0u) << 16);
+        }
+    }
+}
+
 bool repack_tile_major(int wtype, const uint8_t * src, const QMat & dst, int row_off, int rows, cudaStream_t st) {
     if (dst.layout != 1 || (row_off & 15)) { set_error("repack_tile_major: bad destination"); return false; }
     const int K = dst.K, nrec = K / wt_tm_rec_k(wtype);
@@ -191,8 +237,11 @@ bool repack_tile_major(int wtype, const uint8_t * src, const QMat & dst, int row
         if (n_threads == 0) return true;
         uint8_t * out = const_cast<uint8_t *>(reinterpret_cast<const uint8_t *>(dst.base)) + (size_t) (row_off / 16) * nrec * wt_tm_rec_bytes(wtype);
         const unsigned blocks = (unsigned) ((n_threads + 255) / 256);
-        if (wtype == WT_Q4_K) k_repack_tm_kq<WT_Q4_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads);
-        else                  k_repack_tm_kq<WT_Q5_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads);
+        switch (wtype) {
+            case WT_Q4_K: k_repack_tm_kq<WT_Q4_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
+            case WT_Q5_K: k_repack_tm_kq<WT_Q5_K><<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
+            case WT_Q3_K: k_repack_tm_q3k<<<blocks, 256, 0, st>>>(src, out, rows, K, n_threads); break;
+        }
         count_launch();
         return cudaGetLastError() == cudaSuccess;
     }
@@ -413,6 +462,17 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
     const int REC = wt_tm_rec_bytes(W.type), rk = wt_tm_rec_k(W.type), nrec = W.K / rk;
     const int rr = (int) (row & 15), g = rr & 7, up = rr >> 3, i = e % rk;
     const uint8_t * rec = reinterpret_cast<const uint8_t *>(W.base) + ((row >> 4) * nrec + e / rk) * REC;
+    if (W.type == WT_Q3_K) {                                     // dequantize_row_q3_K: (d * sc) * q, each product rounded
+        const int j = i >> 5, l = i & 31, hf = l >> 4, c = (l & 15) >> 2, k = l & 3, r = up + 2 * hf, lane = g * 4 + c;
+        const int sc = (int) reinterpret_cast<const int8_t *>(rec)[4 * (j * 8 + g) + 2 * up + hf];
+        const uint32_t dw = reinterpret_cast<const uint32_t *>(rec + 256)[g];
+        const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dw >> 16) : (dw & 0xffffu))));
+        const uint8_t * sub = rec + 288 + j * wt_tm_sub_bytes(W.type);
+        const int lo = (int) ((reinterpret_cast<const uint32_t *>(sub)[lane] >> (8 * k + 2 * r)) & 3u);
+        const int hb = (int) ((reinterpret_cast<const uint32_t *>(sub + 128)[g * 2 + up] >> l) & 1u);
+        const int q = (lo | (hb << 2)) - 4;
+        return __fmul_rn(__fmul_rn(d, (float) sc), (float) q);
+    }
     if (wt_is_kquant(W.type)) {                                  // dequantize_row_q4_K / _q5_K: (d * sc) * q - dmin * m, each product rounded
         const uint8_t * hdr = rec + 16 * rr;
         const int j = i >> 5, l = i & 31, c = (l & 15) >> 2;
@@ -484,6 +544,8 @@ __device__ __forceinline__ float dequant_elem(const QMat & W, int64_t row, int e
             if (W.type == WT_Q5_K) q |= ((blk[16 + l] >> j) & 1) << 4;
             return d * sc * q - dmin * mn;
         }
+        case WT_Q3_K:
+            return q3k_elem(reinterpret_cast<const uint8_t *>(W.base) + (row * (K >> 8) + (e >> 8)) * 110, e & 255);
     }
     return 0.0f;
 }
@@ -530,7 +592,7 @@ template <int WT> struct GemvSmem;
 template <int WT>
 __device__ __forceinline__ size_t gemv_tok_bytes(int K) {
     if (WT == WT_F16) return (size_t) K * 2;
-    if (WT == WT_Q4_K || WT == WT_Q5_K) return (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
+    if (wt_is_kquant(WT)) return (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
     return (size_t) K + (size_t) (K / 32) * 4;
 }
 
@@ -569,7 +631,7 @@ k_gemv(const GemvK a) {
             const int t = i / K, e = i - t * K;
             reinterpret_cast<__half *>(tokbase + t * tb)[e] = __float2half_rn(xval(t, e));
         }
-    } else if (WT == WT_Q4_K || WT == WT_Q5_K) {
+    } else if (wt_is_kquant(WT)) {
         // quantize_row_q8_K (ggml-quants.c:2768-2805): per 256: iscale = -127/max (signed max-magnitude), q = min(127, nearest(iscale*x)), d = 1/iscale
         const int nsb = K / 256;
         for (int pidx = warp; pidx < a.n_tok * nsb; pidx += 8) {
@@ -688,6 +750,26 @@ k_gemv(const GemvK a) {
                     }
                 }
             }
+        } else if (WT == WT_Q3_K) {
+            constexpr int BLK = 110;
+            const uint8_t * rowp = reinterpret_cast<const uint8_t *>(a.W.base) + (int64_t) row * (K >> 8) * BLK;
+            for (int c = lane; c < K / 8; c += 32) {           // chunk of 8 weights (half of one 16-value scale group): super-block c/32
+                const int sb = c >> 5, e0 = (c & 31) * 8;
+                const uint8_t * blk = rowp + (int64_t) sb * BLK;
+                const int w0 = (int) q3k_q4(blk, e0), w1 = (int) q3k_q4(blk, e0 + 4);
+                const int sc = q3k_scale(blk, e0 >> 4);
+                const float dw = q3k_d(blk);
+#pragma unroll
+                for (int t = 0; t < NT; ++t) {
+                    if (t < a.n_tok) {                           // ggml_vec_dot_q3_K_q8_K: (d_w d_x) * (sc * sumi)
+                        const uint8_t * tp = tokbase + t * tb;
+                        const int * xq = reinterpret_cast<const int *>(tp) + (sb * 256 + e0) / 4;
+                        const float d8 = reinterpret_cast<const float *>(tp + K)[sb];
+                        const int sumi = __dp4a(w0, xq[0], __dp4a(w1, xq[1], 0));
+                        acc[t] = fmaf(dw * d8, (float) (sc * sumi), acc[t]);
+                    }
+                }
+            }
         } else {
             const int64_t rb = (int64_t) row * (K >> 5);
             for (int c = lane; c < K / 8; c += 32) {           // chunk = quarter block
@@ -762,7 +844,7 @@ static void gemv_launch(const GemvK & k, cudaStream_t st) {
     const int K = k.W.K, N = k.W.N;
     size_t tokb;
     if (WT == WT_F16) tokb = (size_t) K * 2;
-    else if (WT == WT_Q4_K || WT == WT_Q5_K) tokb = (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
+    else if (wt_is_kquant(WT)) tokb = (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
     else tokb = (size_t) K + (size_t) (K / 32) * 4;
     tokb = (tokb + 15) & ~size_t(15);
     const size_t smem = tokb * k.n_tok;
@@ -795,6 +877,7 @@ void gemv(const GemvArgs & a, cudaStream_t st) {
         case WT_Q8_0: gemv_nt<WT_Q8_0>(k, st); break;
         case WT_Q4_K: gemv_nt<WT_Q4_K>(k, st); break;
         case WT_Q5_K: gemv_nt<WT_Q5_K>(k, st); break;
+        case WT_Q3_K: gemv_nt<WT_Q3_K>(k, st); break;
         default: set_error("gemv: unsupported weight type %d", a.W.type);
     }
 }
@@ -970,6 +1053,32 @@ k_gemv_mma(const Gemv2K a) {
                 }
             }
         }
+    } else if (WT == WT_Q3_K) {
+        constexpr int BLK = 110;
+        const int nsb = K / 256;
+        const uint32_t * xg = reinterpret_cast<const uint32_t *>(actg);
+        const float * d80 = reinterpret_cast<const float *>(act0 + K), * d81 = reinterpret_cast<const float *>(act1 + K);
+        for (int b = warp; b < K / 32; b += 8) {               // work item = one 32-value sub-block: two k16 products, one per scale
+            const int sb = b >> 3, j = b & 7;
+            const uint32_t b0 = tok_ok ? xg[b * 8 + c] : 0u, b1 = tok_ok ? xg[b * 8 + 4 + c] : 0u;
+            const float x80 = d80[sb], x81 = d81[sb];
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt) {
+                uint32_t af[4], sw = 0; float dw[2];
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const uint8_t * blk = reinterpret_cast<const uint8_t *>(a.W.base) + ((int64_t) rows[2*mt + r] * nsb + sb) * BLK;
+                    af[r] = q3k_q4(blk, 32 * j + 4 * c); af[2 + r] = q3k_q4(blk, 32 * j + 16 + 4 * c);
+                    sw |= ((uint32_t) (q3k_scale(blk, 2 * j) & 0xff) | ((uint32_t) (q3k_scale(blk, 2 * j + 1) & 0xff) << 8)) << (16 * r);
+                    dw[r] = q3k_d(blk);
+                }
+                int si[4]; q3k_sumi(af, b0, b1, sw, si);
+                acc[mt][0] = fmaf(dw[0] * x80, (float) si[0], acc[mt][0]);
+                acc[mt][1] = fmaf(dw[0] * x81, (float) si[1], acc[mt][1]);
+                acc[mt][2] = fmaf(dw[1] * x80, (float) si[2], acc[mt][2]);
+                acc[mt][3] = fmaf(dw[1] * x81, (float) si[3], acc[mt][3]);
+            }
+        }
     } else {
         const int nblk = K >> 5;
         const uint32_t * xg = reinterpret_cast<const uint32_t *>(actg);
@@ -1074,6 +1183,7 @@ void gemv2(const GemvArgs & a, uint8_t * act_scratch, cudaStream_t st) {
         case WT_Q8_0: WB_GEMV2(WT_Q8_0); break;
         case WT_Q4_K: WB_GEMV2(WT_Q4_K); break;
         case WT_Q5_K: WB_GEMV2(WT_Q5_K); break;
+        case WT_Q3_K: WB_GEMV2(WT_Q3_K); break;
         default: set_error("gemv2: unsupported weight type %d", a.W.type); return;
     }
 #undef WB_GEMV2

@@ -70,10 +70,10 @@ bool alloc_qmat(Model & m, int t, int N, int K, QMat & q, bool tile_major = fals
     }
     if (wt_is_kquant(t)) {
         if (K % 256) { set_error("model: K=%d not a multiple of 256 for K-quants", K); return false; }
-        q.base = dalloc(m, (size_t) N * (K / 256) * (t == WT_Q4_K ? 144 : 176));
+        q.base = dalloc(m, (size_t) N * (K / 256) * wt_kq_block_bytes(t));
         return q.base != nullptr;
     }
-    set_error("model: unsupported weight type %d (supported: F32->F16, F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q4_K, Q5_K)", t);
+    set_error("model: unsupported weight type %d (supported: F32->F16, F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q3_K, Q4_K, Q5_K)", t);
     return false;
 }
 
@@ -125,19 +125,19 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
         case 0: m.wtype = WT_F32; break;  case 1: m.wtype = WT_F16; break; case 2: m.wtype = WT_Q4_0; break;
         case 7: m.wtype = WT_Q8_0; break; case 8: m.wtype = WT_Q5_0; break; case 12: m.wtype = WT_Q4_K; break;
         case 13: m.wtype = WT_Q5_K; break; case 3: m.wtype = WT_Q4_1; break; case 9: m.wtype = WT_Q5_1; break;
+        case 11: m.wtype = WT_Q3_K; break;
         // formats without device kernels: expanded on the host at load time, kept in HBM as F16 (wb_dequant_host.h)
-        case 10: host_dq = HT_Q2_K; break;
-        case 11: host_dq = HT_Q3_K; break; case 14: host_dq = HT_Q6_K; break; case 24: host_dq = HT_BF16; break;
+        case 10: host_dq = HT_Q2_K; break; case 14: host_dq = HT_Q6_K; break; case 24: host_dq = HT_BF16; break;
         default: set_error("invalid model (ftype %d is not supported by this engine)", hp.ftype); return false;
     }
     if (wt_is_kquant(m.wtype) && getenv("WB200_KQUANT_AS_F16") && atoi(getenv("WB200_KQUANT_AS_F16")) != 0) {
-        // opt-in: Q4_K / Q5_K expanded to F16 (2 bytes per weight, F16 arithmetic); without it their blocks decode natively (Q8_K activations)
-        host_dq = m.wtype == WT_Q4_K ? HT_Q4_K : HT_Q5_K;
+        // opt-in: K-quants expanded to F16 (2 bytes per weight, F16 arithmetic); without it their blocks decode natively (Q8_K activations)
+        host_dq = m.wtype;                                       // HostDqType ids are the ggml_type ids
     }
     if (host_dq >= 0) {
         m.wtype = WT_F16;
         logf(LOG_WARN, "%s: ftype %d (ggml type %d): matrices are expanded to F16 on the host at load time (%s)\n", __func__, hp.ftype, host_dq,
-             (host_dq == HT_Q4_K || host_dq == HT_Q5_K) ? "WB200_KQUANT_AS_F16" : "no device kernels for this block format");
+             wt_is_kquant(host_dq) ? "WB200_KQUANT_AS_F16" : "no device kernels for this block format");
     }
     const int file_wtype = host_dq >= 0 ? host_dq : m.wtype;
     const int wt = (m.wtype == WT_F32) ? WT_F16 : m.wtype;   // F32 matrices are stored as F16 in HBM
@@ -369,7 +369,7 @@ bool model_load(whisper_model_loader * loader, Model & m, Vocab & vocab, int dev
                 sub.qs = q.qs + boff * wt_qs_bytes(q.type); sub.d = q.d + boff; sub.qh = q.qh ? q.qh + boff : nullptr; sub.m = q.m ? q.m + boff : nullptr;
                 if (!repack_block32_into(q.type, dstage, sub, D.rows, K, 0)) return false;
             } else {
-                const size_t bpr = (size_t) (K / 256) * (q.type == WT_Q4_K ? 144 : 176);
+                const size_t bpr = (size_t) (K / 256) * wt_kq_block_bytes(q.type);
                 WB_CUDA_OK(cudaMemcpy((uint8_t *) q.base + (size_t) D.row_off * bpr, dstage, nbytes, cudaMemcpyDeviceToDevice));
             }
         }

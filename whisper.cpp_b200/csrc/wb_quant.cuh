@@ -2,8 +2,9 @@
 //
 // File side (unchanged legacy ggml container): 32-value blocks block_q4_0 / block_q4_1 / block_q5_0 / block_q5_1 / block_q8_0
 // (ggml/src/ggml-common.h:194-256) and 256-value super-blocks block_q4_K / block_q5_K
-// (ggml-common.h:327-356).  Bit-level meaning follows ggml/src/ggml-quants.c:459-567 (dequantize_row_q4_0,
-// _q5_0, _q8_0), :880-887 (get_scale_min_k4), :1529-1551 (q4_K), :1731-1756 (q5_K).
+// (ggml-common.h:327-356) and block_q3_K (ggml-common.h:310-325).  Bit-level meaning follows
+// ggml/src/ggml-quants.c:459-567 (dequantize_row_q4_0, _q5_0, _q8_0), :880-887 (get_scale_min_k4), :1529-1551 (q4_K),
+// :1731-1756 (q5_K), :1305-1353 (q3_K).
 //
 // HBM side ("planar" layout, built once at load by wb_repack_*): the 18/22/34-byte file blocks are not
 // 16-byte aligned, so every 32-block matrix [N rows][K] is split into three dense arrays
@@ -11,8 +12,7 @@
 //     qh : [N][K/32]       uint32, the fifth bits (Q5_0 / Q5_1)
 //     d  : [N][K/32]       f16 block scale
 //     m  : [N][K/32]       f16 block minimum (Q4_1 / Q5_1: value = q * d + m, q unsigned)
-// Total bytes are identical to the file (18 / 20 / 22 / 24 / 34 per 32 weights).  K-quant super-blocks are 144 / 176
-// bytes = multiples of 16 and are kept verbatim (encoder side; the decoder matrices use the tile-major records below).
+// Total bytes are identical to the file (18 / 20 / 22 / 24 / 34 per 32 weights).  K-quant super-blocks (144 / 176 / 110 bytes) are kept verbatim (encoder side; the decoder matrices use the tile-major records below).
 #pragma once
 #include <cstdint>
 #include <cuda_fp16.h>
@@ -20,7 +20,7 @@
 namespace wb {
 
 // numeric ids are ggml_type (ggml/include/ggml.h:390-405)
-enum WType : int { WT_F32 = 0, WT_F16 = 1, WT_Q4_0 = 2, WT_Q4_1 = 3, WT_Q5_0 = 6, WT_Q5_1 = 7, WT_Q8_0 = 8, WT_Q4_K = 12, WT_Q5_K = 13 };
+enum WType : int { WT_F32 = 0, WT_F16 = 1, WT_Q4_0 = 2, WT_Q4_1 = 3, WT_Q5_0 = 6, WT_Q5_1 = 7, WT_Q8_0 = 8, WT_Q3_K = 11, WT_Q4_K = 12, WT_Q5_K = 13 };
 
 struct QMat {            // one weight matrix resident in HBM
     int   type = WT_F16;
@@ -52,23 +52,39 @@ struct QMat {            // one weight matrix resident in HBM
 //   Q5_K (2816 B): hdr as Q4_K | 8 x sub-block record (320 B): qs as Q4_K | u32 qh[8][2] = { row g, row g+8 } (bit i = fifth bit of q[i])
 // = the file's 16 x 144 / 16 x 176 bytes.  The GEMV splits K per 32-value sub-block (record + 256 + j * 256 / 320); a lane reads 8 bytes
 // of the header: lane 4g + c gets bytes 8 (c & 1) .. +7 of row g + 8 (c >> 1), so a quad holds the 32 header bytes of its two rows.
+// Q3_K (signed values, one integer scale per 16 values, no minimum): one 1824-byte record = a 288-byte header
+//   i8 sc[8 sub-blocks][8 lane groups][4] = { row g: scale of values 0..15, of 16..31; row g + 8: the same }   (256 B; the packed
+//   6-bit scales unpacked to sc - 32 at repack time) | u32 d[8] = { d_g | d_g+8 << 16 }   (32 B)
+// so lane 4g + c finds the four scales of its rows for sub-block j in the word j * 8 + g, and their two d in the word 64 + g; then
+// 8 x sub-block record (192 B): u32 ql[32 lanes]: byte e holds at bits 2r, 2r + 1 the low bit pair of byte e of the lane's A register r
+//   (128 B) | u32 hm[8][2] = { row g, row g+8 } (bit i = hmask bit of q[i], the Q5_K arrangement) (64 B)
+// = 16 x 114 bytes, 3.6 % above the file's 110 (the unpacked scales).
+// (A register r of lane 4g + c: r = 0 / 1 rows g / g + 8 values 4c .. 4c + 3, r = 2 / 3 the same rows, values 16 + 4c .. 16 + 4c + 3.)
 __host__ __device__ inline int wt_tm_rec_bytes(int t) {
-    return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q4_1 ? 320 : t == WT_Q5_1 ? 384 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 : 0;
+    return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q4_1 ? 320 : t == WT_Q5_1 ? 384 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 :
+           t == WT_Q3_K ? 1824 : 0;
 }
-__host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : (t == WT_Q4_K || t == WT_Q5_K) ? 256 : 32; }
-__host__ __device__ inline int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : 320; }      // K-quants: one 32-value sub-block record
+__host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : (t == WT_Q4_K || t == WT_Q5_K || t == WT_Q3_K) ? 256 : 32; }
+// K-quants: bytes of the header and of one 32-value sub-block record
+__host__ __device__ inline int wt_tm_hdr_bytes(int t) { return t == WT_Q3_K ? 288 : 256; }
+__host__ __device__ inline int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : t == WT_Q5_K ? 320 : t == WT_Q3_K ? 192 : 0; }
 __host__ __device__ inline size_t wt_tm_bytes(int t, int N, int K) { return (size_t) ((N + 15) / 16) * (K / wt_tm_rec_k(t)) * wt_tm_rec_bytes(t); }
 
 __host__ __device__ inline int wt_qs_bytes(int t)    { return t == WT_Q8_0 ? 32 : 16; }
 __host__ __device__ inline bool wt_is_block32(int t) { return t == WT_Q4_0 || t == WT_Q5_0 || t == WT_Q8_0 || t == WT_Q4_1 || t == WT_Q5_1; }
 __host__ __device__ inline bool wt_has_min(int t)    { return t == WT_Q4_1 || t == WT_Q5_1; }     // blocks with a minimum: Q8_1 activations
 __host__ __device__ inline bool wt_has_qh(int t)     { return t == WT_Q5_0 || t == WT_Q5_1; }
-__host__ __device__ inline bool wt_is_kquant(int t)  { return t == WT_Q4_K || t == WT_Q5_K; }
+// K-quants: 256-value super-blocks, Q8_K activations.  Q4_K / Q5_K have a minimum term (dmin * m against the activation sums),
+// Q3_K is signed with one integer scale per 16 values
+__host__ __device__ inline bool wt_is_kquant(int t)  { return t == WT_Q4_K || t == WT_Q5_K || t == WT_Q3_K; }
+__host__ __device__ inline bool wt_kq_has_dmin(int t) { return t == WT_Q4_K || t == WT_Q5_K; }
+__host__ __device__ inline int  wt_kq_block_bytes(int t) { return t == WT_Q4_K ? 144 : t == WT_Q5_K ? 176 : t == WT_Q3_K ? 110 : 0; }
 // bytes per weight on disk and in HBM
 __host__ __device__ inline double wt_bpw(int t) {
     switch (t) { case WT_F32: return 4; case WT_F16: return 2; case WT_Q4_0: return 18.0/32; case WT_Q5_0: return 22.0/32;
                  case WT_Q4_1: return 20.0/32; case WT_Q5_1: return 24.0/32;
-                 case WT_Q8_0: return 34.0/32; case WT_Q4_K: return 144.0/256; case WT_Q5_K: return 176.0/256; }
+                 case WT_Q8_0: return 34.0/32; case WT_Q4_K: return 144.0/256; case WT_Q5_K: return 176.0/256;
+                 case WT_Q3_K: return 110.0/256; }
     return 0;
 }
 
@@ -240,6 +256,80 @@ __device__ __forceinline__ void dequant_kq_sub(const uint8_t * __restrict__ blk,
     }
     out[0] = make_uint4(h[0], h[1], h[2], h[3]);   out[1] = make_uint4(h[4], h[5], h[6], h[7]);
     out[2] = make_uint4(h[8], h[9], h[10], h[11]); out[3] = make_uint4(h[12], h[13], h[14], h[15]);
+}
+
+// Q3_K verbatim super-blocks (hmask[32] qs[64] scales[12] f16 d = 110 B).  Blocks are only 2-byte aligned in a row of super-blocks,
+// so words are read as two halves.
+__device__ __forceinline__ uint32_t ld_u32_a2(const uint8_t * p) {
+    const uint16_t * h = reinterpret_cast<const uint16_t *>(p);
+    return (uint32_t) h[0] | ((uint32_t) h[1] << 16);
+}
+// the signed values e .. e + 3 (e % 4 == 0) of a super-block, packed as int8
+__device__ __forceinline__ uint32_t q3k_q4(const uint8_t * blk, int e) {
+    const int n = e >> 7, r = (e >> 5) & 3, l = e & 31;
+    const uint32_t qs = ld_u32_a2(blk + 32 + 32 * n + l), hm = ld_u32_a2(blk + l);
+    return __vsub4(((qs >> (2 * r)) & 0x03030303u) | (((hm >> (4 * n + r)) & 0x01010101u) << 2), 0x04040404u);
+}
+// integer scale of values 16 is .. 16 is + 15 (is = 0 .. 15) from the 12 packed bytes: the 6-bit value - 32
+__device__ __forceinline__ int q3k_scale(const uint8_t * blk, int is) {
+    const int k = is >> 2, i = is & 3;
+    return (int) (((blk[96 + (k & 1) * 4 + i] >> (4 * (k >> 1))) & 0xF) | (((blk[104 + i] >> (2 * k)) & 3) << 4)) - 32;
+}
+__device__ __forceinline__ uint32_t q3k_dbits(const uint8_t * blk) { return *reinterpret_cast<const uint16_t *>(blk + 108); }
+__device__ __forceinline__ float q3k_d(const uint8_t * blk) { return __half2float(__ushort_as_half((unsigned short) q3k_dbits(blk))); }
+// (d * sc) * q of value e (0 .. 255), each product rounded in f32: dequantize_row_q3_K
+__device__ __forceinline__ float q3k_elem(const uint8_t * blk, int e) {
+    const int q = (int) (int8_t) ((q3k_q4(blk, e & ~3) >> (8 * (e & 3))) & 0xffu);
+    return __fmul_rn(__fmul_rn(q3k_d(blk), (float) q3k_scale(blk, e >> 4)), (float) q);
+}
+// sub-block j (32 values) of a Q3_K super-block into 32 halves: the f16 rounding of dequantize_row_q3_K's f32 value
+__device__ __forceinline__ void dequant_q3k_sub(const uint8_t * __restrict__ blk, int j, uint4 (&out)[4]) {
+    const float d = q3k_d(blk);
+    uint32_t h[16];
+#pragma unroll
+    for (int v = 0; v < 8; ++v) {
+        const float dl = __fmul_rn(d, (float) q3k_scale(blk, 2 * j + (v >> 2)));
+        const uint32_t q = q3k_q4(blk, 32 * j + 4 * v);
+        float f[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) f[e] = __fmul_rn(dl, (float) (int) (int8_t) ((q >> (8 * e)) & 0xffu));
+        const __half2 a = __floats2half2_rn(f[0], f[1]), c = __floats2half2_rn(f[2], f[3]);
+        h[2 * v] = *reinterpret_cast<const uint32_t *>(&a); h[2 * v + 1] = *reinterpret_cast<const uint32_t *>(&c);
+    }
+    out[0] = make_uint4(h[0], h[1], h[2], h[3]);   out[1] = make_uint4(h[4], h[5], h[6], h[7]);
+    out[2] = make_uint4(h[8], h[9], h[10], h[11]); out[3] = make_uint4(h[12], h[13], h[14], h[15]);
+}
+
+// bit 2 of byte e of a word -> bit e (the four high bits of Q3_K's stored values q + 4)
+__device__ __forceinline__ uint32_t spread_bit2(uint32_t u) {
+    return ((u >> 2) & 1u) | ((u >> 9) & 2u) | ((u >> 16) & 4u) | ((u >> 23) & 8u);
+}
+// Q3_K tile-major sub-block record -> the four signed A registers of lane (g, c): wl = low bit pairs, wh = hmask bits of rows g, g + 8
+__device__ __forceinline__ void q3k_tm_af(uint32_t wl, uint2 wh, int c, uint32_t (&af)[4]) {
+    af[0] = ( wl       & 0x03030303u) | (spread4_to_bit4(wh.x >> (4 * c)) >> 2);
+    af[1] = ((wl >> 2) & 0x03030303u) | (spread4_to_bit4(wh.y >> (4 * c)) >> 2);
+    af[2] = ((wl >> 4) & 0x03030303u) | (spread4_to_bit4(wh.x >> (16 + 4 * c)) >> 2);
+    af[3] = ((wl >> 6) & 0x03030303u) | (spread4_to_bit4(wh.y >> (16 + 4 * c)) >> 2);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) af[r] = __vsub4(af[r], 0x04040404u);
+}
+// D = A (16 x 16, s8) . B (16 x 8, s8) in s32: A = rows g / g + 8, values 4c .. 4c + 3 of lane 4g + c; B = values 4c .. 4c + 3 of column g
+__device__ __forceinline__ void mma_s8_16816(int (&d)[4], const uint32_t (&a)[2], uint32_t b) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%7,%8,%9,%10};"
+                 : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(b), "r"(0), "r"(0), "r"(0), "r"(0));
+}
+// sumi of one 32-value sub-block against its scales: two k16 integer products, combined with the rows' two 16-value scales each
+// (|result| <= 2 * 16 * 4 * 127 * 32: exact in f32).  sw = the lane's scale word, d[i] as mma_s8_16832's.
+__device__ __forceinline__ void q3k_sumi(const uint32_t (&af)[4], uint32_t b0, uint32_t b1, uint32_t sw, int (&s)[4]) {
+    int lo[4], hi[4];
+    const uint32_t a_lo[2] = { af[0], af[1] }, a_hi[2] = { af[2], af[3] };
+    mma_s8_16816(lo, a_lo, b0);
+    mma_s8_16816(hi, a_hi, b1);
+    const int s0l = (int) (int8_t) (sw & 0xffu), s0h = (int) (int8_t) ((sw >> 8) & 0xffu);
+    const int s1l = (int) (int8_t) ((sw >> 16) & 0xffu), s1h = (int) (int8_t) (sw >> 24);
+    s[0] = s0l * lo[0] + s0h * hi[0]; s[1] = s0l * lo[1] + s0h * hi[1];
+    s[2] = s1l * lo[2] + s1h * hi[2]; s[3] = s1l * lo[3] + s1h * hi[3];
 }
 
 #endif // __CUDACC__

@@ -17,7 +17,7 @@ import numpy as np
 
 F32, F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K = 0, 1, 2, 6, 8, 12, 13
 Q4_1, Q5_1 = 3, 7
-Q2_K, Q3_K, Q6_K, BF16 = 10, 11, 14, 30              # no NumPy quantiser here: pass quantizer= (ggml's own, via the oracle build)
+Q2_K, Q3_K, Q6_K, BF16 = 10, 11, 14, 30              # Q2_K, Q6_K, BF16: no NumPy quantiser here (pass quantizer=, ggml's own via the oracle build)
 FTYPE_OF = {F32: 0, F16: 1, Q4_0: 2, Q8_0: 7, Q5_0: 8, Q4_K: 12, Q5_K: 13, Q4_1: 3, Q5_1: 9, Q2_K: 10, Q3_K: 11, Q6_K: 14, BF16: 24}
 
 CONFIGS = {
@@ -32,6 +32,7 @@ CONFIGS = {
     "test-2l.en":     (51864, 1500, 384, 6, 2, 448, 384, 6, 2, 80),     # NB: 2 text layers + an English vocabulary = "distilled": whisper_full forces no_timestamps (whisper.cpp:7078-7084)
     "test-3l.en":     (51864, 1500, 384, 6, 2, 448, 384, 6, 3, 80),     # 3 text layers: timestamps stay on
     "test-2l-512.en": (51864, 1500, 512, 8, 2, 448, 512, 8, 2, 80),
+    "test-3l-512.en": (51864, 1500, 512, 8, 2, 448, 512, 8, 3, 80),     # a K-quant width (d % 256 == 0) with timestamps on
     "test-2l-multi":  (51866, 1500, 256, 4, 2, 448, 256, 4, 2, 128),
     "small.en":       (51864, 1500, 768, 12, 12, 448, 768, 12, 12, 80),
     "test-2l-768.en": (51864, 1500, 768, 12, 2, 448, 768, 12, 2, 80),     # the small.en width at a depth the CPU reference finishes in seconds
@@ -115,6 +116,8 @@ def quantize(wtype, w):
         return quantize_q1(wtype, x)
     if wtype == Q4_K:
         return quantize_q4_k_simple(w)
+    if wtype == Q3_K:
+        return quantize_q3_k_simple(w)
     raise ValueError(f"synth.quantize: type {wtype} needs an external quantiser (pass quantizer=...)")
 
 
@@ -166,6 +169,41 @@ def quantize_q4_k_simple(w):
     out[:, 4:16] = scales
     for jp in range(4):                                          # 64 values per 32 bytes: low nibbles = sub-block 2jp, high = 2jp+1
         out[:, 16 + 32 * jp:16 + 32 * (jp + 1)] = q[:, 2 * jp] | (q[:, 2 * jp + 1] << 4)
+    return out.tobytes()
+
+
+def _kq_signed_scales(x, qmax, smax):
+    """[nb][256] -> (f16 d [nb], integer scales [nb][16] in 0 .. smax, q [nb][256] in -qmax .. qmax - 1): one scale per 16 values"""
+    g = x.reshape(-1, 16, 16)
+    s = np.abs(g).max(axis=2) / np.float32(qmax)
+    d = (s.max(axis=1) / np.float32(smax)).astype(np.float16).astype(np.float32)
+    sc = np.clip(np.rint(s / np.where(d > 0, d, 1.0)[:, None]), 0, smax).astype(np.int32)
+    step = (d[:, None] * sc).astype(np.float32)
+    q = np.clip(np.rint(g / np.where(step > 0, step, 1.0)[:, :, None]), -qmax, qmax - 1).astype(np.int32)
+    return d, sc, q.reshape(-1, 256)
+
+
+def quantize_q3_k_simple(w):
+    """float32 [rows][k] -> block_q3_K bytes (hmask[32] qs[64] packed 6-bit scales[12] f16 d).  A plain absmax quantiser, not ggml's
+    make_q3_quants search: valid super-blocks that dequantise (dequantize_row_q3_K) close to the input, for the benchmark models; parity
+    tests quantise with the reference's own ggml_quantize_chunk."""
+    x = np.ascontiguousarray(w, np.float32).reshape(-1, 256)
+    nb = x.shape[0]
+    d, sc, q = _kq_signed_scales(x, 4, 31)
+    u = (q + 4).astype(np.uint8)                                 # q = (u & 3) - (hmask bit ? 0 : 4)
+    out = np.zeros((nb, 110), np.uint8)
+    for n in range(2):
+        for r in range(4):
+            v = u[:, 128 * n + 32 * r:128 * n + 32 * r + 32]
+            out[:, 32 + 32 * n:64 + 32 * n] |= (v & 3) << (2 * r)
+            out[:, 0:32] |= (v >> 2) << (4 * n + r)
+    st = (sc + 32).astype(np.uint8)                              # stored 6-bit scale = sc + 32
+    for k in range(4):
+        for i in range(4):
+            v = st[:, 4 * k + i]
+            out[:, 96 + (k & 1) * 4 + i] |= (v & 0xF) << (4 * (k >> 1))
+            out[:, 104 + i] |= (v >> 4) << (2 * k)
+    out[:, 108:110] = d.astype(np.float16).view(np.uint8).reshape(nb, 2)
     return out.tobytes()
 
 
@@ -242,7 +280,7 @@ def write_model(path, config="test-2l.en", wtype=F16, seed=0, sigma=0.02, vocab_
     n_vocab, n_actx, d, n_ah, La, n_tctx, dt, n_th, Lt, n_mels = cfg
     q = quantizer or quantize
     ftype = FTYPE_OF[wtype] + (2000 if wtype not in (F32, F16) else 0)
-    blk = {Q4_0: (32, 18), Q5_0: (32, 22), Q8_0: (32, 34), Q4_1: (32, 20), Q5_1: (32, 24), Q4_K: (256, 144), Q5_K: (256, 176)}.get(wtype)
+    blk = {Q4_0: (32, 18), Q5_0: (32, 22), Q8_0: (32, 34), Q4_1: (32, 20), Q5_1: (32, 24), Q4_K: (256, 144), Q5_K: (256, 176), Q3_K: (256, 110)}.get(wtype)
     pool = None
     if fast_pool:
         prng = np.random.default_rng(seed ^ 0x5EED)
@@ -319,7 +357,7 @@ def cached_model(config, wtype, seed=0, fast_pool=False, tag=None):
     """a synthetic model in the temp directory, written once per box (the multi-GB ones take a while); returns its path"""
     import os
     import tempfile
-    names = {F16: "f16", Q4_0: "q4_0", Q5_0: "q5_0", Q8_0: "q8_0", Q4_K: "q4_k", Q4_1: "q4_1", Q5_1: "q5_1"}
+    names = {F16: "f16", Q4_0: "q4_0", Q5_0: "q5_0", Q8_0: "q8_0", Q4_K: "q4_k", Q4_1: "q4_1", Q5_1: "q5_1", Q3_K: "q3_k"}
     path = os.path.join(tempfile.gettempdir(), "wb200-%s-%s%s.bin" % (config, names[wtype], ("-" + tag) if tag else ""))
     if not os.path.exists(path):
         tmp = path + ".tmp.%d" % os.getpid()
