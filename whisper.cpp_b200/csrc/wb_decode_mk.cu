@@ -29,6 +29,7 @@
 #include "wb_common.h"
 #include "wb_dev.cuh"
 #include "wb_ptx.cuh"
+#include "wb_tm.cuh"
 
 namespace wb {
 
@@ -231,15 +232,15 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const MkView v, const floa
         __syncthreads();
         q = (lane < MK_WARPS) ? SM_STAT[16 + lane] : 0.0f;
         const float rstd = 1.0f / sqrtf(warp_sum(q) / K + a.eps);
+        float4 y = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (act) {
+            const float4 w = __ldg(reinterpret_cast<const float4 *>(ln_w + e0)), b = __ldg(reinterpret_cast<const float4 *>(ln_b + e0));
+            y.x = __fadd_rn(__fmul_rn(__fmul_rn(v.x, rstd), w.x), b.x);
+            y.y = __fadd_rn(__fmul_rn(__fmul_rn(v.y, rstd), w.y), b.y);
+            y.z = __fadd_rn(__fmul_rn(__fmul_rn(v.z, rstd), w.z), b.z);
+            y.w = __fadd_rn(__fmul_rn(__fmul_rn(v.w, rstd), w.w), b.w);
+        }
         if (mk_kq(WT)) {                                         // Q8_K: a super-block is the 256 values of warps 2s, 2s + 1
-            float4 y = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-            if (act) {
-                const float4 w = __ldg(reinterpret_cast<const float4 *>(ln_w + e0)), b = __ldg(reinterpret_cast<const float4 *>(ln_b + e0));
-                y.x = __fadd_rn(__fmul_rn(__fmul_rn(v.x, rstd), w.x), b.x);
-                y.y = __fadd_rn(__fmul_rn(__fmul_rn(v.y, rstd), w.y), b.y);
-                y.z = __fadd_rn(__fmul_rn(__fmul_rn(v.z, rstd), w.z), b.z);
-                y.w = __fadd_rn(__fmul_rn(__fmul_rn(v.w, rstd), w.w), b.w);
-            }
             float amax = fabsf(y.x), mx = y.x;
             q8k_pick(amax, mx, fabsf(y.y), y.y); q8k_pick(amax, mx, fabsf(y.z), y.z); q8k_pick(amax, mx, fabsf(y.w), y.w);
             q8k_warp_max(amax, mx);
@@ -258,12 +259,6 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const MkView v, const floa
                 if (lane == 0 && (warp & 1) == 0) dd[e0 >> 8] = (amax != 0.0f) ? 1.0f / iscale : 0.0f;
             }
         } else if (act) {
-            const float4 w = __ldg(reinterpret_cast<const float4 *>(ln_w + e0)), b = __ldg(reinterpret_cast<const float4 *>(ln_b + e0));
-            float4 y;
-            y.x = __fadd_rn(__fmul_rn(__fmul_rn(v.x, rstd), w.x), b.x);
-            y.y = __fadd_rn(__fmul_rn(__fmul_rn(v.y, rstd), w.y), b.y);
-            y.z = __fadd_rn(__fmul_rn(__fmul_rn(v.z, rstd), w.z), b.z);
-            y.w = __fadd_rn(__fmul_rn(__fmul_rn(v.w, rstd), w.w), b.w);
             if (WT == WT_F16) {
                 const __half2 h0 = __floats2half2_rn(y.x, y.y), h1 = __floats2half2_rn(y.z, y.w);
                 *reinterpret_cast<uint2 *>(reinterpret_cast<__half *>(dst) + (size_t) row * K + e0) = make_uint2(*reinterpret_cast<const uint32_t *>(&h0), *reinterpret_cast<const uint32_t *>(&h1));
@@ -282,36 +277,6 @@ __device__ __noinline__ void mk_lnq(const MkArgs & a, const MkView v, const floa
             }
         }
         __syncthreads();
-    }
-}
-
-// quantise f32 rows (no LayerNorm) into the actq format: one warp per (row, 128 values); followed by a grid barrier
-template <int WT>
-__device__ __noinline__ void mk_q8_rows(const MkView v, const float * src, int K, uint8_t * dst) {
-    const int lane = threadIdx.x & 31, wg = v.ci * MK_WARPS + (threadIdx.x >> 5), nwg = v.nc * MK_WARPS;
-    const int cpr = K >> 7;
-    int row = v.row0 + wg / cpr, ch = wg - (wg / cpr) * cpr;
-    const int drow = nwg / cpr, dch = nwg - drow * cpr;
-    for (; row < v.row0 + v.n_tok; ) {
-        const int e0 = ch * 128 + lane * 4;
-        const float4 y = __ldcg(reinterpret_cast<const float4 *>(src + (size_t) row * K + e0));
-        if (WT == WT_F16) {
-            const __half2 h0 = __floats2half2_rn(y.x, y.y), h1 = __floats2half2_rn(y.z, y.w);
-            *reinterpret_cast<uint2 *>(reinterpret_cast<__half *>(dst) + (size_t) row * K + e0) = make_uint2(*reinterpret_cast<const uint32_t *>(&h0), *reinterpret_cast<const uint32_t *>(&h1));
-        } else {
-            float amax = fmaxf(fmaxf(fabsf(y.x), fabsf(y.y)), fmaxf(fabsf(y.z), fabsf(y.w)));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
-            if (mk_q1(WT)) { mk_q8_1_store4(dst, K, row, e0, lane, y, amax); } else {
-            const float id = (amax != 0.0f) ? __fdividef(127.0f, amax) : 0.0f;
-            const uint32_t q0 = (uint32_t) __float2int_rn(y.x * id) & 0xffu, q1 = (uint32_t) __float2int_rn(y.y * id) & 0xffu;
-            const uint32_t q2 = (uint32_t) __float2int_rn(y.z * id) & 0xffu, q3 = (uint32_t) __float2int_rn(y.w * id) & 0xffu;
-            *reinterpret_cast<uint32_t *>(dst + (size_t) row * K + e0) = q0 | (q1 << 8) | (q2 << 16) | (q3 << 24);
-            if ((lane & 7) == 0) reinterpret_cast<float *>(dst + (size_t) MK_MAXTOK * K)[row * (K >> 5) + (e0 >> 5)] = __half2float(__float2half_rn(amax * (1.0f / 127.0f)));
-            }
-        }
-        row += drow; ch += dch; if (ch >= cpr) { ch -= cpr; ++row; }
     }
 }
 
@@ -367,17 +332,73 @@ __device__ __forceinline__ uint64_t policy_evict_first() { uint64_t p; asm volat
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
+// The activation operand of step b, half h (batch rows 8h ..) from the staged rows: the B fragment (rows >= nt read as zero) and,
+// for batch rows 2c, 2c + 1 (clamped to the last row), the Q8_0 d or Q8_1 {d, s} of the block, or the Q8_K d of the super-block and
+// the sum of the sub-block (mk_store_q comment).
+template <int WT>
+__device__ __forceinline__ TmX mk_xfrag(int b, int h, int g, int c, int SW, int nb, int nt) {
+    TmX x;
+    const bool ok = h * 8 + g < nt;
+    x.b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u;
+    x.b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
+    const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
+    if (mk_kq(WT)) {
+        x.d0 = SM_XD[r0 * nb + (b >> 3)]; x.d1 = SM_XD[r1 * nb + (b >> 3)];
+        if (wt_kq_has_dmin(WT)) {
+            x.s0 = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
+            x.s1 = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
+        }
+    } else if (mk_q1(WT)) {
+        const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[r0 * nb + b], p1 = reinterpret_cast<const __half2 *>(SM_XD)[r1 * nb + b];
+        x.d0 = __low2float(p0); x.s0 = __high2float(p0); x.d1 = __low2float(p1); x.s1 = __high2float(p1);
+    } else if (WT != WT_F16) {
+        x.d0 = SM_XD[r0 * nb + b]; x.d1 = SM_XD[r1 * nb + b];
+    }
+    return x;
+}
+
+// The rows a CTA stages for a GEMV phase.  CTA v.ci serves row group v.ci % NGc of RG rows (8 for the widest F16 matrices: what fits
+// the staging area) as the ci-th of the cg CTAs of that group; nt rows in NH 8-row halves, SW words per staged row.
+struct MkStage { int t_base, nt, NH, SW, ci, cg; uint32_t parity; };
+
+template <int WT>
+__device__ __forceinline__ MkStage mk_rows(const MkView v, int K) {
+    const int rowb = (WT == WT_F16) ? K * 2 : K;
+    const int RG = (16 * (rowb + 16) <= MK_MAXTOK * (MK_ROWB + 16)) ? 16 : 8;
+    const int NGc = (v.n_tok + RG - 1) / RG, grp = v.ci % NGc;
+    MkStage s;
+    s.SW = (rowb >> 2) + 4; s.ci = v.ci / NGc; s.cg = (v.nc - grp + NGc - 1) / NGc;
+    s.t_base = v.row0 + grp * RG; s.nt = min(RG, v.n_tok - grp * RG); s.NH = (s.nt + 7) >> 3;
+    return s;
+}
+// stage the rows of the group: one TMA bulk copy per row (+ one for its block scales), completion on an mbarrier (phase `parity`) that
+// every thread waits for on its own, after it has issued its first weight loads
+template <int WT>
+__device__ __forceinline__ void mk_stage(MkStage & s, const uint8_t * x, int K) {
+    const int tid = threadIdx.x, nb = K >> 5;
+    const int rowb = (WT == WT_F16) ? K * 2 : K;
+    const int ph = SM_FLAG[4];                                   // staging round (mbarrier phase parity)
+    __syncthreads();                                             // everybody has read `ph`; the previous users of the buffer are done
+    s.parity = (uint32_t) ph & 1u;
+    if (tid == 0) {
+        SM_FLAG[4] = ph + 1;
+        mbar_arrive_expect_tx(SM_MBAR, (uint32_t) s.nt * (uint32_t) (rowb + (WT == WT_F16 ? 0 : nb * 4)));
+    }
+    if (tid < s.nt) {
+        asm volatile("fence.proxy.async;" ::: "memory");         // rows were written with ordinary stores (by other CTAs, before the grid barrier)
+        bulk_g2s(SM_XQ + tid * s.SW, x + (size_t) (s.t_base + tid) * rowb, (uint32_t) rowb, SM_MBAR);
+        if (WT != WT_F16)
+            bulk_g2s(SM_XD + tid * nb, reinterpret_cast<const float *>(x + (size_t) MK_MAXTOK * K) + (size_t) (s.t_base + tid) * nb, (uint32_t) nb * 4, SM_MBAR);
+    }
+}
+
 // k-loop of one iteration of mk_gemv for NV tile slots per warp (compile-time: predicated slots made the register allocator spill);
 // leaves the split-K partials of slots j0 .. j0+NV-1 in SM_RED.  KS warps split K of a slot, UB records per slot are requested together
 // (always 16 / 3: the order in which a warp adds up its blocks is part of the result, and a row must not depend on how many tiles its
 // CTA happens to hold).  Four slots in one call hold 12 records + 32 accumulators per lane and spilled (7.4 us per iteration against
 // 2.4 us for three slots): an iteration with four slots makes two calls of two slots, same partials, no spills.
 template <int WT, int NV, int TU, int KS, int UB>
-__device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * wbase, int tile0, int tstep, int nrec, int nb, int SW, int nt, int NH, bool & staged, uint32_t stage_parity, int fb, int j0) {
-    constexpr bool KQ = mk_kq(WT), Q3K = (WT == WT_Q3_K), Q1 = mk_q1(WT);
-    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
-                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : (WT == WT_Q3_K ? 228 : 512)))));   // K-quants: bytes per 32 values
-    constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
+__device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * wbase, int tile0, int tstep, int nrec, int nb, const MkStage s, bool & staged, int fb, int j0) {
     constexpr int RLD = 17;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3, ks = warp & (KS - 1);
     float acc[NV][2][4];
@@ -386,167 +407,32 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 #pragma unroll
         for (int h = 0; h < 2; ++h) { acc[j][h][0] = acc[j][h][1] = acc[j][h][2] = acc[j][h][3] = 0.0f; }
     for (int kb = ks; kb < nrec; kb += KS * UB) {
-        uint4 wq[NV][UB]; uint2 wh[NV][UB]; uint32_t wd[NV][UB]; uint2 wk[NV][UB]; uint2 wm[NV][UB];
+        TmW<WT> w[NV][UB];
 #pragma unroll
         for (int j = 0; j < NV; ++j) {
-            {
-                const uint8_t * tb = wbase + (size_t) ((tile0 + ((j0 + j) / TU) * tstep) * TU + (j0 + j) % TU) * nrec * REC;
+            const size_t r0 = (size_t) ((tile0 + ((j0 + j) / TU) * tstep) * TU + (j0 + j) % TU) * nrec;
 #pragma unroll
-                for (int u = 0; u < UB; ++u) {
-                    if (Q3K) {                                   // Q3_K sub-block record + this lane's scale word and d word
-                        const int bb = min(kb + u * KS, nrec - 1);
-                        const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 288 + (bb & 7) * wt_tm_sub_bytes(WT);
-                        wq[j][u].x = __ldg(reinterpret_cast<const uint32_t *>(rec) + lane);
-                        wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + 128) + g);
-                        wk[j][u] = make_uint2(__ldg(reinterpret_cast<const uint32_t *>(sbp) + (bb & 7) * 8 + g), __ldg(reinterpret_cast<const uint32_t *>(sbp + 256) + g));
-                        continue;
-                    }
-                    if (KQ) {                                    // sub-block record of super-block sb (wb_quant.cuh) + this lane's 8 header bytes
-                        const int bb = min(kb + u * KS, nrec - 1);
-                        const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
-                        const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[j][u].x = q2.x; wq[j][u].y = q2.y;
-                        if (WT == WT_Q5_K) wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + 256) + g);
-                        wk[j][u] = __ldg(reinterpret_cast<const uint2 *>(sbp + 16 * (g + 8 * (c >> 1))) + (c & 1));
-                        continue;
-                    }
-                    const uint8_t * rec = tb + (size_t) min(kb + u * KS, nrec - 1) * REC;
-                    if (WT == WT_F16 || WT == WT_Q8_0) wq[j][u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
-                    else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[j][u].x = q2.x; wq[j][u].y = q2.y; }
-                    if (WT == WT_Q5_0 || WT == WT_Q5_1) wh[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
-                    if (Q1) wm[j][u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB + (WT == WT_Q5_1 ? 64 : 0)) + g);   // {d, d'}, {m, m'}
-                    else if (WT != WT_F16)  wd[j][u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
-                }
-            }
+            for (int u = 0; u < UB; ++u) w[j][u] = tm_load<WT>(wbase, r0, kb + u * KS, nrec, lane, g, c);
         }
-        if (!staged) { mbar_wait(SM_MBAR, stage_parity); staged = true; MK_FINE(1); }     // the rows have landed (this warp's weights are in flight)
+        if (!staged) { mbar_wait(SM_MBAR, s.parity); staged = true; MK_FINE(1); }     // the rows have landed (this warp's weights are in flight)
 #pragma unroll
         for (int u = 0; u < UB; ++u) {
             const int b = kb + u * KS;
             if (b < nrec) {
-                uint32_t bf[2][2]; float dx[2][2], sx[2][2];
+                TmX xf[2];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const bool ok = h * 8 + g < nt;
-                    bf[h][0] = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u;
-                    bf[h][1] = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
-                    dx[h][0] = dx[h][1] = 0.0f;
-                    if (KQ) {                                    // Q8_K: d of the super-block, sum of the sub-block (mk_store_q comment)
-                        const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
-                        dx[h][0] = SM_XD[r0 * nb + (b >> 3)]; dx[h][1] = SM_XD[r1 * nb + (b >> 3)];
-                        if (!Q3K) {
-                            sx[h][0] = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
-                            sx[h][1] = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
-                        }
-                    } else if (Q1) {                             // Q8_1: {d, s} of the block
-                        const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c, nt - 1) * nb + b];
-                        const __half2 p1 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
-                        dx[h][0] = __low2float(p0); sx[h][0] = __high2float(p0); dx[h][1] = __low2float(p1); sx[h][1] = __high2float(p1);
-                    } else if (WT != WT_F16) { dx[h][0] = SM_XD[min(h * 8 + 2 * c, nt - 1) * nb + b]; dx[h][1] = SM_XD[min(h * 8 + 2 * c + 1, nt - 1) * nb + b]; }
-                }
+                for (int h = 0; h < 2; ++h) xf[h] = mk_xfrag<WT>(b, h, g, c, s.SW, nb, s.nt);
 #pragma unroll
                 for (int j = 0; j < NV; ++j) {
-                    if (Q3K) {                                   // signed 3-bit weights; acc += (d_w d_x) (sc_lo sumi_lo + sc_hi sumi_hi)
-                        uint32_t af[4];
-                        q3k_tm_af(wq[j][u].x, wh[j][u], c, af);
-                        const float dw0 = __half2float(__ushort_as_half((unsigned short) (wk[j][u].y & 0xffffu)));
-                        const float dw1 = __half2float(__ushort_as_half((unsigned short) (wk[j][u].y >> 16)));
+                    const TmA f = tm_frag<WT>(w[j][u], b, c);
 #pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            if (h < NH) {
-                                int si[4]; q3k_sumi(af, bf[h][0], bf[h][1], wk[j][u].x, si);
-                                acc[j][h][0] = fmaf(dw0 * dx[h][0], (float) si[0], acc[j][h][0]);
-                                acc[j][h][1] = fmaf(dw0 * dx[h][1], (float) si[1], acc[j][h][1]);
-                                acc[j][h][2] = fmaf(dw1 * dx[h][0], (float) si[2], acc[j][h][2]);
-                                acc[j][h][3] = fmaf(dw1 * dx[h][1], (float) si[3], acc[j][h][3]);
-                            }
-                        }
-                        continue;
-                    }
-                    if (KQ) {                                    // unsigned 4 / 5-bit weights; acc += d_x * (d sc_j * sumi - dmin m_j * sumx) as the chain
-                        uint32_t af[4];
-                        af[0] = wq[j][u].x & 0x0F0F0F0Fu; af[2] = (wq[j][u].x >> 4) & 0x0F0F0F0Fu;
-                        af[1] = wq[j][u].y & 0x0F0F0F0Fu; af[3] = (wq[j][u].y >> 4) & 0x0F0F0F0Fu;
-                        if (WT == WT_Q5_K) {
-                            af[0] |= spread4_to_bit4(wh[j][u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[j][u].x >> (16 + 4 * c));
-                            af[1] |= spread4_to_bit4(wh[j][u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[j][u].y >> (16 + 4 * c));
-                        }
-                        float dl0, ml0, dl1, ml1;
-                        kq_tm_scales(wk[j][u], b & 7, c, dl0, ml0, dl1, ml1);
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            if (h < NH) {
-                                int dd[4]; mma_s8_16832(dd, af, bf[h][0], bf[h][1]);
-                                acc[j][h][0] = fmaf(dx[h][0], fmaf(dl0, (float) dd[0], -ml0 * sx[h][0]), acc[j][h][0]);
-                                acc[j][h][1] = fmaf(dx[h][1], fmaf(dl0, (float) dd[1], -ml0 * sx[h][1]), acc[j][h][1]);
-                                acc[j][h][2] = fmaf(dx[h][0], fmaf(dl1, (float) dd[2], -ml1 * sx[h][0]), acc[j][h][2]);
-                                acc[j][h][3] = fmaf(dx[h][1], fmaf(dl1, (float) dd[3], -ml1 * sx[h][1]), acc[j][h][3]);
-                            }
-                        }
-                        continue;
-                    }
-                    if (Q1) {                                    // unsigned 4 / 5-bit weights; acc += (d_w d_x) sumi, then m_w s_x
-                        uint32_t af[4];
-                        af[0] = wq[j][u].x & 0x0F0F0F0Fu; af[2] = (wq[j][u].x >> 4) & 0x0F0F0F0Fu;
-                        af[1] = wq[j][u].y & 0x0F0F0F0Fu; af[3] = (wq[j][u].y >> 4) & 0x0F0F0F0Fu;
-                        if (WT == WT_Q5_1) {
-                            af[0] |= spread4_to_bit4(wh[j][u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[j][u].x >> (16 + 4 * c));
-                            af[1] |= spread4_to_bit4(wh[j][u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[j][u].y >> (16 + 4 * c));
-                        }
-                        const float dw0 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].x & 0xffffu)));
-                        const float dw1 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].x >> 16)));
-                        const float mw0 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].y & 0xffffu)));
-                        const float mw1 = __half2float(__ushort_as_half((unsigned short) (wm[j][u].y >> 16)));
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            if (h < NH) {
-                                int dd[4]; mma_s8_16832(dd, af, bf[h][0], bf[h][1]);
-                                acc[j][h][0] = fmaf(mw0, sx[h][0], fmaf(dw0 * dx[h][0], (float) dd[0], acc[j][h][0]));
-                                acc[j][h][1] = fmaf(mw0, sx[h][1], fmaf(dw0 * dx[h][1], (float) dd[1], acc[j][h][1]));
-                                acc[j][h][2] = fmaf(mw1, sx[h][0], fmaf(dw1 * dx[h][0], (float) dd[2], acc[j][h][2]));
-                                acc[j][h][3] = fmaf(mw1, sx[h][1], fmaf(dw1 * dx[h][1], (float) dd[3], acc[j][h][3]));
-                            }
-                        }
-                        continue;
-                    }
-                    {
-                        uint32_t af[4];
-                        float dw0 = 0.0f, dw1 = 0.0f;
-                        if (WT == WT_F16 || WT == WT_Q8_0) { af[0] = wq[j][u].x; af[1] = wq[j][u].y; af[2] = wq[j][u].z; af[3] = wq[j][u].w; }
-                        else {
-                            uint32_t lo0 = wq[j][u].x & 0x0F0F0F0Fu, hi0 = (wq[j][u].x >> 4) & 0x0F0F0F0Fu, lo1 = wq[j][u].y & 0x0F0F0F0Fu, hi1 = (wq[j][u].y >> 4) & 0x0F0F0F0Fu;
-                            if (WT == WT_Q5_0) {
-                                lo0 |= spread4_to_bit4(wh[j][u].x >> (4 * c)); hi0 |= spread4_to_bit4(wh[j][u].x >> (16 + 4 * c));
-                                lo1 |= spread4_to_bit4(wh[j][u].y >> (4 * c)); hi1 |= spread4_to_bit4(wh[j][u].y >> (16 + 4 * c));
-                                af[0] = __vsub4(lo0, 0x10101010u); af[2] = __vsub4(hi0, 0x10101010u);
-                                af[1] = __vsub4(lo1, 0x10101010u); af[3] = __vsub4(hi1, 0x10101010u);
-                            } else {
-                                af[0] = __vsub4(lo0, 0x08080808u); af[2] = __vsub4(hi0, 0x08080808u);
-                                af[1] = __vsub4(lo1, 0x08080808u); af[3] = __vsub4(hi1, 0x08080808u);
-                            }
-                        }
-                        if (WT != WT_F16) {
-                            dw0 = __half2float(__ushort_as_half((unsigned short) (wd[j][u] & 0xffffu)));
-                            dw1 = __half2float(__ushort_as_half((unsigned short) (wd[j][u] >> 16)));
-                        }
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            if (h < NH) {
-                                if (WT == WT_F16) mma_f16_16816(acc[j][h], af, bf[h][0], bf[h][1]);
-                                else {
-                                    int dd[4]; mma_s8_16832(dd, af, bf[h][0], bf[h][1]);
-                                    acc[j][h][0] = fmaf(dw0 * dx[h][0], (float) dd[0], acc[j][h][0]);
-                                    acc[j][h][1] = fmaf(dw0 * dx[h][1], (float) dd[1], acc[j][h][1]);
-                                    acc[j][h][2] = fmaf(dw1 * dx[h][0], (float) dd[2], acc[j][h][2]);
-                                    acc[j][h][3] = fmaf(dw1 * dx[h][1], (float) dd[3], acc[j][h][3]);
-                                }
-                            }
-                        }
-                    }
+                    for (int h = 0; h < 2; ++h)
+                        if (h < s.NH) tm_dot<WT>(f, xf[h], acc[j][h]);
                 }
             }
         }
     }
-    if (!staged) { mbar_wait(SM_MBAR, stage_parity); staged = true; }
+    if (!staged) { mbar_wait(SM_MBAR, s.parity); staged = true; }
     // split-K partials -> smem: red[tile slot j][warp][row][batch row]
 #pragma unroll
     for (int j = 0; j < NV; ++j)
@@ -572,41 +458,20 @@ __device__ __forceinline__ void mk_gemv_kloop(const MkArgs & a, const uint8_t * 
 // quantised-row format FC2 consumes (one warp = one Q8_0 block of one row) -- no f32 round trip, no extra phase.
 template <int WT, bool PAIR>
 __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, const MkEpi & e, int fb = -1) {
-    constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;             // bytes of the qs part of a record
-    constexpr int RK = (WT == WT_F16) ? 16 : 32;                 // K values per record
     constexpr int UB = 3;                                        // records whose loads are issued together
     constexpr int TP = MK_TP;                                    // tile slots per iteration
     constexpr int TU = PAIR ? 2 : 1;                             // tiles per unit of distribution
     constexpr int RLD = 17;                                      // row stride of the reduction buffer (16 batch rows + pad)
     const int N = W.N, K = W.K;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3;
-    const int n_tiles = (N + 15) >> 4, nrec = K / RK, nb = K >> 5;
-    const int rowb = (WT == WT_F16) ? K * 2 : K, SW = (rowb >> 2) + 4;
-    const int RG = (16 * (rowb + 16) <= MK_MAXTOK * (MK_ROWB + 16)) ? 16 : 8;   // rows per CTA (what fits the staging area)
-    const int NGc = (v.n_tok + RG - 1) / RG;
-    const int grp = v.ci % NGc, ci = v.ci / NGc, cg = (v.nc - grp + NGc - 1) / NGc;   // row group, index / count of its CTAs
-    const int t_base = v.row0 + grp * RG, nt = min(RG, v.n_tok - grp * RG), NH = (nt + 7) >> 3;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n_tiles = (N + 15) >> 4, nrec = K / wt_tm_step_k(WT), nb = K >> 5;
+    MkStage s = mk_rows<WT>(v, K);
+    const int ci = s.ci, cg = s.cg, t_base = s.t_base, nt = s.nt;
     const int n_units = n_tiles / TU;                            // PAIR: N is a multiple of 32
     const int upc = ci < n_units ? (n_units - ci + cg - 1) / cg : 0;            // units of this CTA: ci, ci + cg, ...
     const int n_it = (upc * TU + TP - 1) / TP, upi = n_it ? (upc + n_it - 1) / n_it : 0;   // iterations, units per iteration (even split)
     MK_FINE(0);
-    uint32_t stage_parity;
-    {   // stage the rows of the group: one TMA bulk copy per row (+ one for its block scales), completion on an mbarrier that every
-        // thread waits for on its own, after it has issued its first weight loads
-        const int ph = SM_FLAG[4];                               // staging round (mbarrier phase parity)
-        __syncthreads();                                         // everybody has read `ph`; the previous users of the buffer are done
-        stage_parity = (uint32_t) ph & 1u;
-        if (tid == 0) {
-            SM_FLAG[4] = ph + 1;
-            mbar_arrive_expect_tx(SM_MBAR, (uint32_t) nt * (uint32_t) (rowb + (WT == WT_F16 ? 0 : nb * 4)));
-        }
-        if (tid < nt) {
-            asm volatile("fence.proxy.async;" ::: "memory");     // rows were written with ordinary stores (by other CTAs, before the grid barrier)
-            bulk_g2s(SM_XQ + tid * SW, x + (size_t) (t_base + tid) * rowb, (uint32_t) rowb, SM_MBAR);
-            if (WT != WT_F16)
-                bulk_g2s(SM_XD + tid * nb, reinterpret_cast<const float *>(x + (size_t) MK_MAXTOK * K) + (size_t) (t_base + tid) * nb, (uint32_t) nb * 4, SM_MBAR);
-        }
-    }
+    mk_stage<WT>(s, x, K);
     bool staged = false;
     for (int it = 0; it < n_it; ++it) {
         const int u0 = it * upi, nv = TU * (min(upc, u0 + upi) - u0);           // valid tile slots of this iteration (CTA-uniform)
@@ -614,18 +479,18 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
             const uint8_t * wbase = reinterpret_cast<const uint8_t *>(W.base);
             const int unit0 = ci + u0 * cg;                      // slot j holds tile (unit0 + (j / TU) * cg) * TU + j % TU
             switch (nv) {
-                case 1: if (!PAIR) { mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
-                case 2: mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break;
+                case 1: if (!PAIR) { mk_gemv_kloop<WT, 1, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 0); break; }
+                case 2: mk_gemv_kloop<WT, 2, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 0); break;
                 case 3:
                     if (!PAIR && (mk_kq(WT) || WT == WT_Q5_1)) {     // K-quant records carry a header share (and Q5_K fifth bits), Q5_1 ones fifth bits and minima: two slots + one
-                        mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0);
-                        mk_gemv_kloop<WT, 1, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 2);
+                        mk_gemv_kloop<WT, 2, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 0);
+                        mk_gemv_kloop<WT, 1, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 2);
                         break;
                     }
-                    if (!PAIR) { mk_gemv_kloop<WT, 3, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0); break; }
+                    if (!PAIR) { mk_gemv_kloop<WT, 3, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 0); break; }
                 default:                                         // four slots: two passes of two (see mk_gemv_kloop)
-                    mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 0);
-                    mk_gemv_kloop<WT, 2, TU, 16, 3>(a, wbase, unit0, cg, nrec, nb, SW, nt, NH, staged, stage_parity, fb, 2);
+                    mk_gemv_kloop<WT, 2, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 0);
+                    mk_gemv_kloop<WT, 2, TU, 16, UB>(a, wbase, unit0, cg, nrec, nb, s, staged, fb, 2);
                     break;
             }
         }
@@ -676,7 +541,7 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
         __syncthreads();                                         // SM_RED is rewritten by the next iteration
         if (it == 0) MK_FINE(4);
     }
-    if (!staged) mbar_wait(SM_MBAR, stage_parity);               // a CTA without tiles still waits for its copies before the area is reused
+    if (!staged) mbar_wait(SM_MBAR, s.parity);                   // a CTA without tiles still waits for its copies before the area is reused
     MK_FINE(5);
 }
 
@@ -686,181 +551,32 @@ __device__ __noinline__ void mk_gemv(const MkArgs & a, const MkView v, const QMa
 // is one accumulator over the blocks in ascending order: independent of the batch.
 template <int WT>
 __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, const QMat & W, const uint8_t * x, float * out) {
-    constexpr bool KQ = mk_kq(WT), Q3K = (WT == WT_Q3_K), Q1 = mk_q1(WT);
-    constexpr int REC = (WT == WT_Q4_0 || WT == WT_Q4_K) ? 288 : ((WT == WT_Q5_0 || WT == WT_Q5_K) ? 352 : (WT == WT_Q8_0 ? 544 :
-                        (WT == WT_Q4_1 ? 320 : (WT == WT_Q5_1 ? 384 : (WT == WT_Q3_K ? 228 : 512)))));
-    constexpr int QSB = (WT == WT_Q8_0) ? 512 : 256;
-    constexpr int RK = (WT == WT_F16) ? 16 : 32;
     constexpr int UB = 8;
     const int N = W.N, K = W.K;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, c = lane & 3;
-    const int n_tiles = (N + 15) >> 4, nrec = K / RK, nb = K >> 5;
-    const int rowb = (WT == WT_F16) ? K * 2 : K, SW = (rowb >> 2) + 4;
-    const int RG = (16 * (rowb + 16) <= MK_MAXTOK * (MK_ROWB + 16)) ? 16 : 8;
-    const int NGc = (v.n_tok + RG - 1) / RG;
-    const int grp = v.ci % NGc, ci = v.ci / NGc, cg = (v.nc - grp + NGc - 1) / NGc;
-    const int t_base = v.row0 + grp * RG, nt = min(RG, v.n_tok - grp * RG), NH = (nt + 7) >> 3;
-    uint32_t stage_parity;
-    {
-        const int ph = SM_FLAG[4];
-        __syncthreads();
-        stage_parity = (uint32_t) ph & 1u;
-        if (tid == 0) {
-            SM_FLAG[4] = ph + 1;
-            mbar_arrive_expect_tx(SM_MBAR, (uint32_t) nt * (uint32_t) (rowb + (WT == WT_F16 ? 0 : nb * 4)));
-        }
-        if (tid < nt) {
-            asm volatile("fence.proxy.async;" ::: "memory");
-            bulk_g2s(SM_XQ + tid * SW, x + (size_t) (t_base + tid) * rowb, (uint32_t) rowb, SM_MBAR);
-            if (WT != WT_F16)
-                bulk_g2s(SM_XD + tid * nb, reinterpret_cast<const float *>(x + (size_t) MK_MAXTOK * K) + (size_t) (t_base + tid) * nb, (uint32_t) nb * 4, SM_MBAR);
-        }
-    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, c = lane & 3;
+    const int n_tiles = (N + 15) >> 4, nrec = K / wt_tm_step_k(WT), nb = K >> 5;
+    MkStage s = mk_rows<WT>(v, K);
+    mk_stage<WT>(s, x, K);
     bool staged = false;
     const uint8_t * wbase = reinterpret_cast<const uint8_t *>(W.base);
-    for (int tile = ci * MK_WARPS + warp; tile < n_tiles; tile += cg * MK_WARPS) {
+    for (int tile = s.ci * MK_WARPS + warp; tile < n_tiles; tile += s.cg * MK_WARPS) {
         float acc[2][4];
 #pragma unroll
         for (int h = 0; h < 2; ++h) { acc[h][0] = acc[h][1] = acc[h][2] = acc[h][3] = 0.0f; }
-        const uint8_t * tb = wbase + (size_t) tile * nrec * REC;
+        const size_t r0 = (size_t) tile * nrec;
         for (int kb = 0; kb < nrec; kb += UB) {
-            uint4 wq[UB]; uint2 wh[UB]; uint32_t wd[UB]; uint2 wk[UB]; uint2 wm[UB];
+            TmW<WT> w[UB];
 #pragma unroll
-            for (int u = 0; u < UB; ++u) {
-                if (Q3K) {
-                    const int bb = min(kb + u, nrec - 1);
-                    const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 288 + (bb & 7) * wt_tm_sub_bytes(WT);
-                    wq[u].x = __ldg(reinterpret_cast<const uint32_t *>(rec) + lane);
-                    wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + 128) + g);
-                    wk[u] = make_uint2(__ldg(reinterpret_cast<const uint32_t *>(sbp) + (bb & 7) * 8 + g), __ldg(reinterpret_cast<const uint32_t *>(sbp + 256) + g));
-                    continue;
-                }
-                if (KQ) {
-                    const int bb = min(kb + u, nrec - 1);
-                    const uint8_t * sbp = tb + (size_t) (bb >> 3) * (8 * REC), * rec = sbp + 256 + (bb & 7) * wt_tm_sub_bytes(WT);
-                    const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[u].x = q2.x; wq[u].y = q2.y;
-                    if (WT == WT_Q5_K) wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + 256) + g);
-                    wk[u] = __ldg(reinterpret_cast<const uint2 *>(sbp + 16 * (g + 8 * (c >> 1))) + (c & 1));
-                    continue;
-                }
-                const uint8_t * rec = tb + (size_t) min(kb + u, nrec - 1) * REC;
-                if (WT == WT_F16 || WT == WT_Q8_0) wq[u] = __ldg(reinterpret_cast<const uint4 *>(rec) + lane);
-                else { const uint2 q2 = __ldg(reinterpret_cast<const uint2 *>(rec) + lane); wq[u].x = q2.x; wq[u].y = q2.y; }
-                if (WT == WT_Q5_0 || WT == WT_Q5_1) wh[u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB) + g);
-                if (Q1) wm[u] = __ldg(reinterpret_cast<const uint2 *>(rec + QSB + (WT == WT_Q5_1 ? 64 : 0)) + g);
-                else if (WT != WT_F16)  wd[u] = __ldg(reinterpret_cast<const uint32_t *>(rec + QSB + (WT == WT_Q5_0 ? 64 : 0)) + g);
-            }
-            if (!staged) { mbar_wait(SM_MBAR, stage_parity); staged = true; }
+            for (int u = 0; u < UB; ++u) w[u] = tm_load<WT>(wbase, r0, kb + u, nrec, lane, g, c);
+            if (!staged) { mbar_wait(SM_MBAR, s.parity); staged = true; }
 #pragma unroll
             for (int u = 0; u < UB; ++u) {
                 const int b = kb + u;
-                if (Q3K && b < nrec) {
-                    uint32_t af[4];
-                    q3k_tm_af(wq[u].x, wh[u], c, af);
-                    const float dw0 = __half2float(__ushort_as_half((unsigned short) (wk[u].y & 0xffffu)));
-                    const float dw1 = __half2float(__ushort_as_half((unsigned short) (wk[u].y >> 16)));
+                if (b < nrec) {
+                    const TmA f = tm_frag<WT>(w[u], b, c);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (h < NH) {
-                            const bool ok = h * 8 + g < nt;
-                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
-                            const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
-                            const float dx0 = SM_XD[r0 * nb + (b >> 3)], dx1 = SM_XD[r1 * nb + (b >> 3)];
-                            int si[4]; q3k_sumi(af, b0, b1, wk[u].x, si);
-                            acc[h][0] = fmaf(dw0 * dx0, (float) si[0], acc[h][0]);
-                            acc[h][1] = fmaf(dw0 * dx1, (float) si[1], acc[h][1]);
-                            acc[h][2] = fmaf(dw1 * dx0, (float) si[2], acc[h][2]);
-                            acc[h][3] = fmaf(dw1 * dx1, (float) si[3], acc[h][3]);
-                        }
-                    }
-                } else if (KQ && b < nrec) {
-                    uint32_t af[4];
-                    af[0] = wq[u].x & 0x0F0F0F0Fu; af[2] = (wq[u].x >> 4) & 0x0F0F0F0Fu;
-                    af[1] = wq[u].y & 0x0F0F0F0Fu; af[3] = (wq[u].y >> 4) & 0x0F0F0F0Fu;
-                    if (WT == WT_Q5_K) {
-                        af[0] |= spread4_to_bit4(wh[u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[u].x >> (16 + 4 * c));
-                        af[1] |= spread4_to_bit4(wh[u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[u].y >> (16 + 4 * c));
-                    }
-                    float dl0, ml0, dl1, ml1;
-                    kq_tm_scales(wk[u], b & 7, c, dl0, ml0, dl1, ml1);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (h < NH) {
-                            const bool ok = h * 8 + g < nt;
-                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
-                            const int r0 = min(h * 8 + 2 * c, nt - 1), r1 = min(h * 8 + 2 * c + 1, nt - 1);
-                            const float dx0 = SM_XD[r0 * nb + (b >> 3)], dx1 = SM_XD[r1 * nb + (b >> 3)];
-                            const float sx0 = (float) reinterpret_cast<const short *>(SM_XD + r0 * nb + (nb >> 3))[b];
-                            const float sx1 = (float) reinterpret_cast<const short *>(SM_XD + r1 * nb + (nb >> 3))[b];
-                            int dd[4]; mma_s8_16832(dd, af, b0, b1);
-                            acc[h][0] = fmaf(dx0, fmaf(dl0, (float) dd[0], -ml0 * sx0), acc[h][0]);
-                            acc[h][1] = fmaf(dx1, fmaf(dl0, (float) dd[1], -ml0 * sx1), acc[h][1]);
-                            acc[h][2] = fmaf(dx0, fmaf(dl1, (float) dd[2], -ml1 * sx0), acc[h][2]);
-                            acc[h][3] = fmaf(dx1, fmaf(dl1, (float) dd[3], -ml1 * sx1), acc[h][3]);
-                        }
-                    }
-                } else if (Q1 && b < nrec) {
-                    uint32_t af[4];
-                    af[0] = wq[u].x & 0x0F0F0F0Fu; af[2] = (wq[u].x >> 4) & 0x0F0F0F0Fu;
-                    af[1] = wq[u].y & 0x0F0F0F0Fu; af[3] = (wq[u].y >> 4) & 0x0F0F0F0Fu;
-                    if (WT == WT_Q5_1) {
-                        af[0] |= spread4_to_bit4(wh[u].x >> (4 * c)); af[2] |= spread4_to_bit4(wh[u].x >> (16 + 4 * c));
-                        af[1] |= spread4_to_bit4(wh[u].y >> (4 * c)); af[3] |= spread4_to_bit4(wh[u].y >> (16 + 4 * c));
-                    }
-                    const float dw0 = __half2float(__ushort_as_half((unsigned short) (wm[u].x & 0xffffu)));
-                    const float dw1 = __half2float(__ushort_as_half((unsigned short) (wm[u].x >> 16)));
-                    const float mw0 = __half2float(__ushort_as_half((unsigned short) (wm[u].y & 0xffffu)));
-                    const float mw1 = __half2float(__ushort_as_half((unsigned short) (wm[u].y >> 16)));
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (h < NH) {
-                            const bool ok = h * 8 + g < nt;
-                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
-                            const __half2 p0 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c, nt - 1) * nb + b];
-                            const __half2 p1 = reinterpret_cast<const __half2 *>(SM_XD)[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
-                            int dd[4]; mma_s8_16832(dd, af, b0, b1);
-                            acc[h][0] = fmaf(mw0, __high2float(p0), fmaf(dw0 * __low2float(p0), (float) dd[0], acc[h][0]));
-                            acc[h][1] = fmaf(mw0, __high2float(p1), fmaf(dw0 * __low2float(p1), (float) dd[1], acc[h][1]));
-                            acc[h][2] = fmaf(mw1, __high2float(p0), fmaf(dw1 * __low2float(p0), (float) dd[2], acc[h][2]));
-                            acc[h][3] = fmaf(mw1, __high2float(p1), fmaf(dw1 * __low2float(p1), (float) dd[3], acc[h][3]));
-                        }
-                    }
-                } else if (!KQ && !Q1 && b < nrec) {
-                    uint32_t af[4];
-                    float dw0 = 0.0f, dw1 = 0.0f;
-                    if (WT == WT_F16 || WT == WT_Q8_0) { af[0] = wq[u].x; af[1] = wq[u].y; af[2] = wq[u].z; af[3] = wq[u].w; }
-                    else {
-                        uint32_t lo0 = wq[u].x & 0x0F0F0F0Fu, hi0 = (wq[u].x >> 4) & 0x0F0F0F0Fu, lo1 = wq[u].y & 0x0F0F0F0Fu, hi1 = (wq[u].y >> 4) & 0x0F0F0F0Fu;
-                        if (WT == WT_Q5_0) {
-                            lo0 |= spread4_to_bit4(wh[u].x >> (4 * c)); hi0 |= spread4_to_bit4(wh[u].x >> (16 + 4 * c));
-                            lo1 |= spread4_to_bit4(wh[u].y >> (4 * c)); hi1 |= spread4_to_bit4(wh[u].y >> (16 + 4 * c));
-                            af[0] = __vsub4(lo0, 0x10101010u); af[2] = __vsub4(hi0, 0x10101010u);
-                            af[1] = __vsub4(lo1, 0x10101010u); af[3] = __vsub4(hi1, 0x10101010u);
-                        } else {
-                            af[0] = __vsub4(lo0, 0x08080808u); af[2] = __vsub4(hi0, 0x08080808u);
-                            af[1] = __vsub4(lo1, 0x08080808u); af[3] = __vsub4(hi1, 0x08080808u);
-                        }
-                    }
-                    if (WT != WT_F16) {
-                        dw0 = __half2float(__ushort_as_half((unsigned short) (wd[u] & 0xffffu)));
-                        dw1 = __half2float(__ushort_as_half((unsigned short) (wd[u] >> 16)));
-                    }
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (h < NH) {
-                            const bool ok = h * 8 + g < nt;
-                            const uint32_t b0 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + c] : 0u, b1 = ok ? SM_XQ[(h * 8 + g) * SW + b * 8 + 4 + c] : 0u;
-                            if (WT == WT_F16) mma_f16_16816(acc[h], af, b0, b1);
-                            else {
-                                const float dx0 = SM_XD[min(h * 8 + 2 * c, nt - 1) * nb + b], dx1 = SM_XD[min(h * 8 + 2 * c + 1, nt - 1) * nb + b];
-                                int dd[4]; mma_s8_16832(dd, af, b0, b1);
-                                acc[h][0] = fmaf(dw0 * dx0, (float) dd[0], acc[h][0]);
-                                acc[h][1] = fmaf(dw0 * dx1, (float) dd[1], acc[h][1]);
-                                acc[h][2] = fmaf(dw1 * dx0, (float) dd[2], acc[h][2]);
-                                acc[h][3] = fmaf(dw1 * dx1, (float) dd[3], acc[h][3]);
-                            }
-                        }
-                    }
+                    for (int h = 0; h < 2; ++h)
+                        if (h < s.NH) tm_dot<WT>(f, mk_xfrag<WT>(b, h, g, c, s.SW, nb, s.nt), acc[h]);
                 }
             }
         }
@@ -870,10 +586,10 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int row = tile * 16 + g + (i >> 1) * 8, tl = h * 8 + 2 * c + (i & 1);
-                if (tl < nt && row < N) out[(size_t) (t_base + tl) * N + row] = acc[h][i];
+                if (tl < s.nt && row < N) out[(size_t) (s.t_base + tl) * N + row] = acc[h][i];
             }
     }
-    if (!staged) mbar_wait(SM_MBAR, stage_parity);
+    if (!staged) mbar_wait(SM_MBAR, s.parity);
 }
 
 // ---- attention -----------------------------------------------------------------------------------------------------------

@@ -117,21 +117,20 @@ __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restri
     if (WT == WT_Q8_0) reinterpret_cast<uint4 *>(rec)[lane] = make_uint4(word(b0, r0, c), word(b1, r1, c), word(b0, r0, 4 + c), word(b1, r1, 4 + c));
     else               reinterpret_cast<uint2 *>(rec)[lane] = make_uint2(word(b0, r0, c), word(b1, r1, c));
     if (c == 0) {                                                // lanes 0,4,..: the per-row fields of rows g and g+8
-        const int qsb = (WT == WT_Q8_0) ? 512 : 256;
         auto d16 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[0] | ((uint32_t) blk[1] << 8)) : 0u; };
         if (wt_has_min(WT)) {                                    // Q4_1 / Q5_1: file block d, m, (qh), qs
             auto m16 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[2] | ((uint32_t) blk[3] << 8)) : 0u; };
             if (WT == WT_Q5_1) {
                 auto h32 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[4] | ((uint32_t) blk[5] << 8) | ((uint32_t) blk[6] << 16) | ((uint32_t) blk[7] << 24)) : 0u; };
-                reinterpret_cast<uint2 *>(rec + qsb)[g] = make_uint2(h32(b0, r0), h32(b1, r1));
+                reinterpret_cast<uint2 *>(rec + wt_tm_qs_bytes(WT))[g] = make_uint2(h32(b0, r0), h32(b1, r1));
             }
-            reinterpret_cast<uint2 *>(rec + qsb + (WT == WT_Q5_1 ? 64 : 0))[g] = make_uint2(d16(b0, r0) | (d16(b1, r1) << 16), m16(b0, r0) | (m16(b1, r1) << 16));
+            reinterpret_cast<uint2 *>(rec + wt_tm_d_off(WT))[g] = make_uint2(d16(b0, r0) | (d16(b1, r1) << 16), m16(b0, r0) | (m16(b1, r1) << 16));
         } else if (WT == WT_Q5_0) {
             auto h32 = [&](const uint8_t * blk, int64_t r) -> uint32_t { return r < rows ? ((uint32_t) blk[2] | ((uint32_t) blk[3] << 8) | ((uint32_t) blk[4] << 16) | ((uint32_t) blk[5] << 24)) : 0u; };
-            reinterpret_cast<uint2 *>(rec + qsb)[g] = make_uint2(h32(b0, r0), h32(b1, r1));
-            reinterpret_cast<uint32_t *>(rec + qsb + 64)[g] = d16(b0, r0) | (d16(b1, r1) << 16);
+            reinterpret_cast<uint2 *>(rec + wt_tm_qs_bytes(WT))[g] = make_uint2(h32(b0, r0), h32(b1, r1));
+            reinterpret_cast<uint32_t *>(rec + wt_tm_d_off(WT))[g] = d16(b0, r0) | (d16(b1, r1) << 16);
         } else {
-            reinterpret_cast<uint32_t *>(rec + qsb)[g] = d16(b0, r0) | (d16(b1, r1) << 16);
+            reinterpret_cast<uint32_t *>(rec + wt_tm_d_off(WT))[g] = d16(b0, r0) | (d16(b1, r1) << 16);
         }
     }
 }
@@ -140,7 +139,7 @@ __global__ void k_repack_tm(const uint8_t * __restrict__ src, uint8_t * __restri
 template <int WT>
 __global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int rows, int K, int64_t n_threads) {
     constexpr int BLK = (WT == WT_Q4_K) ? 144 : 176, QOFF = (WT == WT_Q4_K) ? 16 : 48;
-    const int REC = wt_tm_rec_bytes(WT), SUB = wt_tm_sub_bytes(WT), nsub = K / 32, nsb = K / 256;
+    const int REC = wt_tm_rec_bytes(WT), nsub = K / 32, nsb = K / 256;
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_threads) return;
     const int lane = (int) (i & 31), g = lane >> 2, c = lane & 3;
@@ -148,7 +147,7 @@ __global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __res
     const int b = (int) (rb % nsub), sb = b >> 3, j = b & 7;
     const int64_t tile = rb / nsub;
     uint8_t * sbp = dst + (tile * nsb + sb) * REC;
-    uint8_t * rec = sbp + 256 + j * SUB;
+    uint8_t * rec = sbp + wt_tm_sub_off(WT, j);
     const int64_t r0 = tile * 16 + g, r1 = r0 + 8;
     auto blk = [&](int64_t r) { return src + (r * nsb + sb) * BLK; };
     // bytes 4c .. 4c+3 of the row's 32 values in the Q4_0 order: byte i = q[i] | q[i + 16] << 4
@@ -173,9 +172,10 @@ __global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __res
             for (int e = 0; e < 32; ++e) h |= (uint32_t) ((qh[e] >> j) & 1) << e;
             return h;
         };
-        reinterpret_cast<uint2 *>(rec + 256)[g] = make_uint2(hbits(r0), hbits(r1));
+        reinterpret_cast<uint2 *>(rec + wt_tm_qs_bytes(WT))[g] = make_uint2(hbits(r0), hbits(r1));
     }
     if (j == 0) {                                                // header: 16 bytes (d, dmin, scales) of each of the 16 rows
+        static_assert(WT_TM_KQ_HDR_ROW == 16, "two lanes per header row");
         const int64_t r = tile * 16 + (lane >> 1);
         uint32_t w[2] = { 0u, 0u };
         if (r < rows) memcpy(w, blk(r) + 8 * (lane & 1), 8);
@@ -187,7 +187,7 @@ __global__ void k_repack_tm_kq(const uint8_t * __restrict__ src, uint8_t * __res
 // header (scale words lane and lane + 32, d words of lanes 0 .. 7)
 __global__ void k_repack_tm_q3k(const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int rows, int K, int64_t n_threads) {
     constexpr int BLK = 110;
-    const int REC = wt_tm_rec_bytes(WT_Q3_K), SUB = wt_tm_sub_bytes(WT_Q3_K), nsub = K / 32, nsb = K / 256;
+    const int REC = wt_tm_rec_bytes(WT_Q3_K), nsub = K / 32, nsb = K / 256;
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_threads) return;
     const int lane = (int) (i & 31), g = lane >> 2, c = lane & 3;
@@ -195,7 +195,7 @@ __global__ void k_repack_tm_q3k(const uint8_t * __restrict__ src, uint8_t * __re
     const int b = (int) (rb % nsub), sb = b >> 3, j = b & 7;
     const int64_t tile = rb / nsub;
     uint8_t * sbp = dst + (tile * nsb + sb) * REC;
-    uint8_t * rec = sbp + 288 + j * SUB;
+    uint8_t * rec = sbp + wt_tm_sub_off(WT_Q3_K, j);
     const int64_t r0 = tile * 16 + g, r1 = r0 + 8;
     auto blk = [&](int64_t r) { return src + (r * nsb + sb) * BLK; };
     // stored values q + 4 of values 32 j + v .. + 3 of row r; rows >= N: 0 (their scales are 0)
@@ -212,7 +212,7 @@ __global__ void k_repack_tm_q3k(const uint8_t * __restrict__ src, uint8_t * __re
             for (int v = 0; v < 32; v += 4) h |= spread_bit2(uval4(r, v)) << v;
             return h;
         };
-        reinterpret_cast<uint2 *>(rec + 128)[g] = make_uint2(hbits(r0), hbits(r1));
+        reinterpret_cast<uint2 *>(rec + wt_tm_qs_bytes(WT_Q3_K))[g] = make_uint2(hbits(r0), hbits(r1));
     }
     if (j == 0) {                                                // header
         auto sc = [&](int64_t r, int is) -> uint32_t { return r < rows ? (uint32_t) (q3k_scale(blk(r), is) & 0xff) : 0u; };
@@ -224,7 +224,7 @@ __global__ void k_repack_tm_q3k(const uint8_t * __restrict__ src, uint8_t * __re
         }
         if (lane < 8) {
             const int64_t ra = tile * 16 + lane, rb8 = ra + 8;
-            reinterpret_cast<uint32_t *>(sbp + 256)[lane] = (ra < rows ? q3k_dbits(blk(ra)) : 0u) | ((rb8 < rows ? q3k_dbits(blk(rb8)) : 0u) << 16);
+            reinterpret_cast<uint32_t *>(sbp + WT_TM_Q3K_D_OFF)[lane] = (ra < rows ? q3k_dbits(blk(ra)) : 0u) | ((rb8 < rows ? q3k_dbits(blk(rb8)) : 0u) << 16);
         }
     }
 }
@@ -465,23 +465,23 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
     if (W.type == WT_Q3_K) {                                     // dequantize_row_q3_K: (d * sc) * q, each product rounded
         const int j = i >> 5, l = i & 31, hf = l >> 4, c = (l & 15) >> 2, k = l & 3, r = up + 2 * hf, lane = g * 4 + c;
         const int sc = (int) reinterpret_cast<const int8_t *>(rec)[4 * (j * 8 + g) + 2 * up + hf];
-        const uint32_t dw = reinterpret_cast<const uint32_t *>(rec + 256)[g];
+        const uint32_t dw = reinterpret_cast<const uint32_t *>(rec + WT_TM_Q3K_D_OFF)[g];
         const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dw >> 16) : (dw & 0xffffu))));
-        const uint8_t * sub = rec + 288 + j * wt_tm_sub_bytes(W.type);
+        const uint8_t * sub = rec + wt_tm_sub_off(W.type, j);
         const int lo = (int) ((reinterpret_cast<const uint32_t *>(sub)[lane] >> (8 * k + 2 * r)) & 3u);
-        const int hb = (int) ((reinterpret_cast<const uint32_t *>(sub + 128)[g * 2 + up] >> l) & 1u);
+        const int hb = (int) ((reinterpret_cast<const uint32_t *>(sub + wt_tm_qs_bytes(W.type))[g * 2 + up] >> l) & 1u);
         const int q = (lo | (hb << 2)) - 4;
         return __fmul_rn(__fmul_rn(d, (float) sc), (float) q);
     }
     if (wt_is_kquant(W.type)) {                                  // dequantize_row_q4_K / _q5_K: (d * sc) * q - dmin * m, each product rounded
-        const uint8_t * hdr = rec + 16 * rr;
+        const uint8_t * hdr = rec + WT_TM_KQ_HDR_ROW * rr;
         const int j = i >> 5, l = i & 31, c = (l & 15) >> 2;
         int sc, mn; kq_scale_min(j, hdr + 4, sc, mn);
         const float d = __half2float(*reinterpret_cast<const __half *>(hdr)), dmin = __half2float(*reinterpret_cast<const __half *>(hdr + 2));
-        const uint8_t * sub = rec + 256 + j * wt_tm_sub_bytes(W.type);
+        const uint8_t * sub = rec + wt_tm_sub_off(W.type, j);
         const uint32_t w = reinterpret_cast<const uint32_t *>(sub)[(g * 4 + c) * 2 + up];
         int q = (int) ((w >> (8 * (l & 3) + 4 * (l >> 4))) & 0xFu);
-        if (W.type == WT_Q5_K) q |= (int) ((reinterpret_cast<const uint32_t *>(sub + 256)[g * 2 + up] >> l) & 1u) << 4;
+        if (W.type == WT_Q5_K) q |= (int) ((reinterpret_cast<const uint32_t *>(sub + wt_tm_qs_bytes(W.type))[g * 2 + up] >> l) & 1u) << 4;
         return __fsub_rn(__fmul_rn(__fmul_rn(d, (float) sc), (float) q), __fmul_rn(dmin, (float) mn));
     }
     if (W.type == WT_F16) {
@@ -489,18 +489,17 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
         const uint32_t w = reinterpret_cast<const uint32_t *>(rec)[(g * 4 + c) * 4 + k];
         return __half2float(__ushort_as_half((unsigned short) ((i & 1) ? (w >> 16) : (w & 0xffffu))));
     }
-    const int qsb = (W.type == WT_Q8_0) ? 512 : 256;
     if (wt_has_min(W.type)) {                                    // dequantize_row_q4_1 / _q5_1: q * d + m
-        const uint2 dm = reinterpret_cast<const uint2 *>(rec + qsb + (W.type == WT_Q5_1 ? 64 : 0))[g];
+        const uint2 dm = reinterpret_cast<const uint2 *>(rec + wt_tm_d_off(W.type))[g];
         const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dm.x >> 16) : (dm.x & 0xffffu))));
         const float m = __half2float(__ushort_as_half((unsigned short) (up ? (dm.y >> 16) : (dm.y & 0xffffu))));
         const int c = (i & 15) >> 2;
         const uint32_t w = reinterpret_cast<const uint32_t *>(rec)[(g * 4 + c) * 2 + up];
         int q = (int) ((w >> (8 * (i & 3) + 4 * (i >> 4))) & 0xFu);
-        if (W.type == WT_Q5_1) q |= (int) ((reinterpret_cast<const uint32_t *>(rec + 256)[g * 2 + up] >> i) & 1u) << 4;
+        if (W.type == WT_Q5_1) q |= (int) ((reinterpret_cast<const uint32_t *>(rec + wt_tm_qs_bytes(W.type))[g * 2 + up] >> i) & 1u) << 4;
         return __fadd_rn(__fmul_rn((float) q, d), m);
     }
-    const uint32_t dd = reinterpret_cast<const uint32_t *>(rec + qsb + (W.type == WT_Q5_0 ? 64 : 0))[g];
+    const uint32_t dd = reinterpret_cast<const uint32_t *>(rec + wt_tm_d_off(W.type))[g];
     const float d = __half2float(__ushort_as_half((unsigned short) (up ? (dd >> 16) : (dd & 0xffffu))));
     if (W.type == WT_Q8_0) {
         const int c = (i & 15) >> 2, k = up + ((i >> 4) << 1);
@@ -510,7 +509,7 @@ __device__ __forceinline__ float dequant_elem_tm(const QMat & W, int64_t row, in
     const int c = (i & 15) >> 2;
     const uint32_t w = reinterpret_cast<const uint32_t *>(rec)[(g * 4 + c) * 2 + up];
     int q = (int) ((w >> (8 * (i & 3) + 4 * (i >> 4))) & 0xFu);
-    if (W.type == WT_Q5_0) { const uint32_t qh = reinterpret_cast<const uint32_t *>(rec + 256)[g * 2 + up]; q |= (int) ((qh >> i) & 1u) << 4; return d * (float) (q - 16); }
+    if (W.type == WT_Q5_0) { const uint32_t qh = reinterpret_cast<const uint32_t *>(rec + wt_tm_qs_bytes(W.type))[g * 2 + up]; q |= (int) ((qh >> i) & 1u) << 4; return d * (float) (q - 16); }
     return d * (float) (q - 8);
 }
 __device__ __forceinline__ float dequant_elem(const QMat & W, int64_t row, int e) {

@@ -35,6 +35,16 @@ struct QMat {            // one weight matrix resident in HBM
                                    // persistent GEMM; each value is the f16 rounding of the exact d * (q - off)); nullptr = expand per launch
 };
 
+__host__ __device__ inline int wt_qs_bytes(int t)    { return t == WT_Q8_0 ? 32 : 16; }
+__host__ __device__ constexpr bool wt_is_block32(int t) { return t == WT_Q4_0 || t == WT_Q5_0 || t == WT_Q8_0 || t == WT_Q4_1 || t == WT_Q5_1; }
+__host__ __device__ constexpr bool wt_has_min(int t)    { return t == WT_Q4_1 || t == WT_Q5_1; }     // blocks with a minimum: Q8_1 activations
+__host__ __device__ constexpr bool wt_has_qh(int t)     { return t == WT_Q5_0 || t == WT_Q5_1; }
+// K-quants: 256-value super-blocks, Q8_K activations.  Q4_K / Q5_K have a minimum term (dmin * m against the activation sums),
+// Q3_K is signed with one integer scale per 16 values
+__host__ __device__ constexpr bool wt_is_kquant(int t)  { return t == WT_Q4_K || t == WT_Q5_K || t == WT_Q3_K; }
+__host__ __device__ constexpr bool wt_kq_has_dmin(int t) { return t == WT_Q4_K || t == WT_Q5_K; }
+__host__ __device__ inline int  wt_kq_block_bytes(int t) { return t == WT_Q4_K ? 144 : t == WT_Q5_K ? 176 : t == WT_Q3_K ? 110 : 0; }
+
 // "Tile-major" layout of the decoder matrices (persistent decode kernel, wb_decode_mk.cu).  The matrix is cut into tiles of
 // 16 output rows; for every tile and every 32-value block (F16: every 16 values) there is ONE contiguous record holding the
 // operands in the register order of the warp-level MMA (lane = 4*g + c reads rows g and g+8 of the tile):
@@ -60,25 +70,30 @@ struct QMat {            // one weight matrix resident in HBM
 //   (128 B) | u32 hm[8][2] = { row g, row g+8 } (bit i = hmask bit of q[i], the Q5_K arrangement) (64 B)
 // = 16 x 114 bytes, 3.6 % above the file's 110 (the unpacked scales).
 // (A register r of lane 4g + c: r = 0 / 1 rows g / g + 8 values 4c .. 4c + 3, r = 2 / 3 the same rows, values 16 + 4c .. 16 + 4c + 3.)
-__host__ __device__ inline int wt_tm_rec_bytes(int t) {
+// These accessors are the only place the sizes and offsets are written down: the repack writers (wb_kernels.cu), the element reader
+// dequant_elem_tm and the decode kernel's record reader (wb_tm.cuh) take them from here.
+__host__ __device__ constexpr int wt_tm_rec_bytes(int t) {
     return t == WT_Q4_0 ? 288 : t == WT_Q5_0 ? 352 : t == WT_Q4_1 ? 320 : t == WT_Q5_1 ? 384 : t == WT_Q8_0 ? 544 : t == WT_F16 ? 512 : t == WT_Q4_K ? 2304 : t == WT_Q5_K ? 2816 :
            t == WT_Q3_K ? 1824 : 0;
 }
-__host__ __device__ inline int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : (t == WT_Q4_K || t == WT_Q5_K || t == WT_Q3_K) ? 256 : 32; }
-// K-quants: bytes of the header and of one 32-value sub-block record
-__host__ __device__ inline int wt_tm_hdr_bytes(int t) { return t == WT_Q3_K ? 288 : 256; }
-__host__ __device__ inline int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : t == WT_Q5_K ? 320 : t == WT_Q3_K ? 192 : 0; }
+__host__ __device__ constexpr int wt_tm_rec_k(int t)     { return t == WT_F16 ? 16 : wt_is_kquant(t) ? 256 : 32; }
+// one MMA step: the K values a warp multiplies per record (K-quants: per sub-block record), and the record bytes per step
+__host__ __device__ constexpr int wt_tm_step_k(int t)     { return t == WT_F16 ? 16 : 32; }
+__host__ __device__ constexpr int wt_tm_step_bytes(int t) { return wt_tm_rec_bytes(t) / (wt_tm_rec_k(t) / wt_tm_step_k(t)); }
+// inside a record (K-quants: inside a sub-block record): the qs words (Q3_K: ql), then the fifth-bit words (Q3_K: hm), then the
+// 32-block types' f16 d[8][2] or {d, m} words
+__host__ __device__ constexpr int wt_tm_qs_bytes(int t)   { return t == WT_Q8_0 ? 512 : t == WT_Q3_K ? 128 : 256; }
+__host__ __device__ constexpr int wt_tm_d_off(int t)      { return wt_tm_qs_bytes(t) + (wt_has_qh(t) ? 64 : 0); }
+// K-quants: the header (Q4_K / Q5_K: 16 bytes per row; Q3_K: the scale words, then u32 d[8] at WT_TM_Q3K_D_OFF), then the
+// 32-value sub-block records
+constexpr int WT_TM_KQ_HDR_ROW = 16, WT_TM_Q3K_D_OFF = 256;
+__host__ __device__ constexpr int wt_tm_hdr_bytes(int t) { return t == WT_Q3_K ? WT_TM_Q3K_D_OFF + 32 : 16 * WT_TM_KQ_HDR_ROW; }
+__host__ __device__ constexpr int wt_tm_sub_bytes(int t) { return t == WT_Q4_K ? 256 : t == WT_Q5_K ? 320 : t == WT_Q3_K ? 192 : 0; }
+__host__ __device__ constexpr int wt_tm_sub_off(int t, int j) { return wt_tm_hdr_bytes(t) + j * wt_tm_sub_bytes(t); }
 __host__ __device__ inline size_t wt_tm_bytes(int t, int N, int K) { return (size_t) ((N + 15) / 16) * (K / wt_tm_rec_k(t)) * wt_tm_rec_bytes(t); }
-
-__host__ __device__ inline int wt_qs_bytes(int t)    { return t == WT_Q8_0 ? 32 : 16; }
-__host__ __device__ inline bool wt_is_block32(int t) { return t == WT_Q4_0 || t == WT_Q5_0 || t == WT_Q8_0 || t == WT_Q4_1 || t == WT_Q5_1; }
-__host__ __device__ inline bool wt_has_min(int t)    { return t == WT_Q4_1 || t == WT_Q5_1; }     // blocks with a minimum: Q8_1 activations
-__host__ __device__ inline bool wt_has_qh(int t)     { return t == WT_Q5_0 || t == WT_Q5_1; }
-// K-quants: 256-value super-blocks, Q8_K activations.  Q4_K / Q5_K have a minimum term (dmin * m against the activation sums),
-// Q3_K is signed with one integer scale per 16 values
-__host__ __device__ inline bool wt_is_kquant(int t)  { return t == WT_Q4_K || t == WT_Q5_K || t == WT_Q3_K; }
-__host__ __device__ inline bool wt_kq_has_dmin(int t) { return t == WT_Q4_K || t == WT_Q5_K; }
-__host__ __device__ inline int  wt_kq_block_bytes(int t) { return t == WT_Q4_K ? 144 : t == WT_Q5_K ? 176 : t == WT_Q3_K ? 110 : 0; }
+static_assert(wt_tm_step_bytes(WT_Q4_K) == 288 && wt_tm_step_bytes(WT_Q5_K) == 352 && wt_tm_step_bytes(WT_Q3_K) == 228, "K-quant records");
+static_assert(wt_tm_sub_off(WT_Q5_K, 8) == wt_tm_rec_bytes(WT_Q5_K) && wt_tm_sub_off(WT_Q3_K, 8) == wt_tm_rec_bytes(WT_Q3_K), "K-quant records");
+static_assert(wt_tm_d_off(WT_Q5_1) + 64 == wt_tm_rec_bytes(WT_Q5_1) && wt_tm_d_off(WT_Q8_0) + 32 == wt_tm_rec_bytes(WT_Q8_0), "32-block records");
 // bytes per weight on disk and in HBM
 __host__ __device__ inline double wt_bpw(int t) {
     switch (t) { case WT_F32: return 4; case WT_F16: return 2; case WT_Q4_0: return 18.0/32; case WT_Q5_0: return 22.0/32;
