@@ -466,6 +466,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
     const int * d_tok = dints.p, * d_pos = dints.p + R, * d_cell = dints.p + 2 * R, * d_slot = dints.p + 3 * R, * d_nkv = dints.p + 4 * R, * d_row = dints.p + 5 * R;
     const int * d_cap = dints.p + 7 * R, * d_idx = dints.p + 8 * R;
 
+    auto chain_gemv = [&](const GemvArgs & a) { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); };
     dec_embed(m->d_te, m->d_pe, d_tok, d_pos, n, d, dx.p, st);
     if (use_mk) {
         MkArgs a;
@@ -521,23 +522,23 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
         __half * vc = kv_v.p + (size_t) l * n_cells * d;
         { GemvArgs a; a.W = L.qkv; a.x = dx.p; a.n_tok = n; a.ln_w = L.ln0.w; a.ln_b = L.ln0.b; a.eps = hp.eps;      // whisper.cpp:2536-2599
           a.bias = L.qkv_bias; a.scale = L.qkv_scale; a.out = dqkv.p; a.k_cache = kc; a.v_cache = vc; a.cells = d_cell; a.kv_d = d;
-          { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }
+          chain_gemv(a); }
         attn_self_decode(dqkv.p, 3*d, kc, vc, d_idx, ld_idx, d_nkv, n, H, d, dattn.p, d, st);                            // 2603-2625
-        { GemvArgs a; a.W = L.o; a.x = dattn.p; a.n_tok = n; a.bias = L.o_bias; a.res = dx.p; a.out = dx.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }    // 2647-2659
+        { GemvArgs a; a.W = L.o; a.x = dattn.p; a.n_tok = n; a.bias = L.o_bias; a.res = dx.p; a.out = dx.p; chain_gemv(a); }    // 2647-2659
         { GemvArgs a; a.W = L.cq; a.x = dx.p; a.n_tok = n; a.ln_w = L.lnc.w; a.ln_b = L.lnc.b; a.eps = hp.eps;        // 2661-2681
-          a.bias = L.cq_bias; a.out = dq2.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }
+          a.bias = L.cq_bias; a.out = dq2.p; chain_gemv(a); }
         if (pass_capture && dtw_layer_mask[l] != 0u &&               // DTW rows: keep the alignment-head queries of this layer
             !dtw_capture_launch(dq2.p, d, d_cap, n, dtw_layer_mask[l], dtw_layer_head0[l], dtw_q.p, dtw_cap_rows, st)) return false;
         attn_cross_decode(dq2.p, d, kv_cross.p + (size_t) l * Tp * d, kv_cross.p + (size_t) (Lt + l) * Tp * d, d_slot,
                           (int64_t) 2 * Lt * Tp * d, n_keys, n, H, d, kq_scale, xpart.p, xcnt.p, dattn.p, d, st);       // 2688-2705
-        { GemvArgs a; a.W = L.co; a.x = dattn.p; a.n_tok = n; a.bias = L.co_bias; a.res = dx.p; a.out = dx.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }  // 2754-2766
+        { GemvArgs a; a.W = L.co; a.x = dattn.p; a.n_tok = n; a.bias = L.co_bias; a.res = dx.p; a.out = dx.p; chain_gemv(a); }  // 2754-2766
         { GemvArgs a; a.W = L.fc1; a.x = dx.p; a.n_tok = n; a.ln_w = L.lnm.w; a.ln_b = L.lnm.b; a.eps = hp.eps;       // 2770-2794
-          a.bias = L.fc1_bias; a.act = 1; a.out = dh.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }
-        { GemvArgs a; a.W = L.fc2; a.x = dh.p; a.n_tok = n; a.bias = L.fc2_bias; a.res = dx.p; a.out = dx.p; { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); } }   // 2797-2806
+          a.bias = L.fc1_bias; a.act = 1; a.out = dh.p; chain_gemv(a); }
+        { GemvArgs a; a.W = L.fc2; a.x = dh.p; a.n_tok = n; a.bias = L.fc2_bias; a.res = dx.p; a.out = dx.p; chain_gemv(a); }   // 2797-2806
     }
     if (any_logits) {
         GemvArgs a; a.W = m->d_te; a.x = dx.p; a.n_tok = n; a.ln_w = m->d_ln.w; a.ln_b = m->d_ln.b; a.eps = hp.eps; a.out = dlogits.p;   // 2811-2827
-        if (!use_mk) { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); }      // the persistent kernel already wrote dlogits
+        if (!use_mk) chain_gemv(a);      // the persistent kernel already wrote dlogits
         if (samp) {
             SampCfg c = *samp; c.mask = samp_mask.p;
             if (draw_stride > 1) WB_CUDA_OK(cudaMemcpyAsync(ddraws.p, hdraws, (size_t) n * draw_stride * sizeof(double), cudaMemcpyHostToDevice, st));

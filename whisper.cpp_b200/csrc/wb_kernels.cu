@@ -584,15 +584,40 @@ struct GemvK {
     __half * k_cache, * v_cache; const int * cells; int kv_d;
 };
 
-template <int WT> struct GemvSmem;
-
-// shared-memory carve-up (dynamic): per token  xq int8[K] | xd float[K/32] (block32) / xd float[K/256] + bs int[K/32] (K-quant)
-// or half[K] for F16.
-template <int WT>
-__device__ __forceinline__ size_t gemv_tok_bytes(int K) {
-    if (WT == WT_F16) return (size_t) K * 2;
-    if (wt_is_kquant(WT)) return (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
-    return (size_t) K + (size_t) (K / 32) * 4;
+// quantize_row_q8_K (ggml-quants.c:2768-2805) of super-block sb of one activation row (layout: act_tok_stride), by one warp: per 256
+// values iscale = -127/max (signed max-magnitude), q = min(127, nearest(iscale*x)), d = 1/iscale, and the sums of the eight 32-value
+// sub-blocks.  xval(i): value i of the row.
+template <class F>
+__device__ __forceinline__ void q8k_quant_sb(F xval, uint8_t * tp, int K, int sb, int lane) {
+    int8_t * xq = reinterpret_cast<int8_t *>(tp);
+    float * xd = reinterpret_cast<float *>(tp + K);
+    int *   bs = reinterpret_cast<int *>(tp + K + (K / 256) * 4);
+    float v[8]; float amax = 0.0f, mx = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { v[j] = xval(sb * 256 + j * 32 + lane); const float av = fabsf(v[j]); if (av > amax) { amax = av; mx = v[j]; } }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float oa = __shfl_xor_sync(0xffffffffu, amax, o), om = __shfl_xor_sync(0xffffffffu, mx, o);
+        if (oa > amax) { amax = oa; mx = om; }
+    }
+    if (amax == 0.0f) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) xq[sb * 256 + j * 32 + lane] = 0;
+        if (lane == 0) xd[sb] = 0.0f;
+        if (lane < 8) bs[sb * 8 + lane] = 0;
+        return;
+    }
+    const float iscale = -127.0f / mx;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        int q = __float2int_rn(iscale * v[j]); q = min(127, q);
+        xq[sb * 256 + j * 32 + lane] = (int8_t) q;
+        int ssum = q;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
+        if (lane == 0) bs[sb * 8 + j] = ssum;
+    }
+    if (lane == 0) xd[sb] = 1.0f / iscale;
 }
 
 template <int WT, int NT>
@@ -602,7 +627,7 @@ k_gemv(const GemvK a) {
     const int K = a.W.K, N = a.W.N;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint8_t * tokbase = sm;
-    const size_t tb = (gemv_tok_bytes<WT>(K) + 15) & ~size_t(15);
+    const size_t tb = act_tok_stride(WT, K);                 // shared memory: one activation row per token
 
     // ---------------------------------------------------------------- prologue: (LN) + activation quantisation
     // LayerNorm statistics: one warp per token (two passes, like the reference); quantisation: the (token, block) pairs are
@@ -631,40 +656,10 @@ k_gemv(const GemvK a) {
             reinterpret_cast<__half *>(tokbase + t * tb)[e] = __float2half_rn(xval(t, e));
         }
     } else if (wt_is_kquant(WT)) {
-        // quantize_row_q8_K (ggml-quants.c:2768-2805): per 256: iscale = -127/max (signed max-magnitude), q = min(127, nearest(iscale*x)), d = 1/iscale
         const int nsb = K / 256;
         for (int pidx = warp; pidx < a.n_tok * nsb; pidx += 8) {
-            const int t = pidx / nsb, sb = pidx - t * nsb;
-            uint8_t * tp = tokbase + t * tb;
-            int8_t * xq = reinterpret_cast<int8_t *>(tp);
-            float * xd = reinterpret_cast<float *>(tp + K);
-            int *   bs = reinterpret_cast<int *>(tp + K + nsb * 4);
-            float v[8]; float amax = 0.0f, mx = 0.0f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { v[j] = xval(t, sb * 256 + j * 32 + lane); const float av = fabsf(v[j]); if (av > amax) { amax = av; mx = v[j]; } }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float oa = __shfl_xor_sync(0xffffffffu, amax, o), om = __shfl_xor_sync(0xffffffffu, mx, o);
-                if (oa > amax) { amax = oa; mx = om; }
-            }
-            if (amax == 0.0f) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) xq[sb * 256 + j * 32 + lane] = 0;
-                if (lane == 0) xd[sb] = 0.0f;
-                if (lane < 8) bs[sb * 8 + lane] = 0;
-                continue;
-            }
-            const float iscale = -127.0f / mx;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                int q = __float2int_rn(iscale * v[j]); q = min(127, q);
-                xq[sb * 256 + j * 32 + lane] = (int8_t) q;
-                int ssum = q;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
-                if (lane == 0) bs[sb * 8 + j] = ssum;
-            }
-            if (lane == 0) xd[sb] = 1.0f / iscale;
+            const int t = pidx / nsb;
+            q8k_quant_sb([&](int i) { return xval(t, i); }, tokbase + t * tb, K, pidx - t * nsb, lane);
         }
     } else {
         const int nb = K / 32;
@@ -841,12 +836,7 @@ k_gemv(const GemvK a) {
 template <int WT, int NT>
 static void gemv_launch(const GemvK & k, cudaStream_t st) {
     const int K = k.W.K, N = k.W.N;
-    size_t tokb;
-    if (WT == WT_F16) tokb = (size_t) K * 2;
-    else if (wt_is_kquant(WT)) tokb = (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
-    else tokb = (size_t) K + (size_t) (K / 32) * 4;
-    tokb = (tokb + 15) & ~size_t(15);
-    const size_t smem = tokb * k.n_tok;
+    const size_t smem = act_tok_stride(WT, K) * k.n_tok;
     auto kern = k_gemv<WT, NT>;
     if (smem > 48 * 1024) ensure_dyn_smem(reinterpret_cast<const void *>(kern), smem);
     int grid = (N + 7) / 8;                  // one row per warp per pass
@@ -887,7 +877,7 @@ void gemv(const GemvArgs & a, cudaStream_t st) {
 //  over the weights:   D[16 rows][8 tokens] (i32) = W_q[16][32] . X_q8[32][8]   -- exactly one 32-value quant block --
 //  followed by acc += D * d_w[row] * d_x[token] in f32: the same integer-dot + block-scale arithmetic as the reference's
 //  vec_dot_q*_q8_0 (ggml-cpu/quants.c:365-406) and the dp4a kernel above; only the f32 summation order differs.
-//  One CTA = 32 output rows (two m16 tiles); its 8 warps split K and reduce through shared memory.
+//  One CTA = 16 or 32 output rows (one or two m16 tiles); its 8 warps split K and reduce through shared memory.
 // =====================================================================================================================
 template <int MODE>   // 0: Q8_0 blocks  1: Q8_K super-blocks  2: f16  3: Q8_1 blocks
 __global__ void __launch_bounds__(256)
@@ -913,38 +903,7 @@ k_act_quant(const float * __restrict__ x, int K, const float * __restrict__ ln_w
     if (MODE == 2) {
         for (int i = tid; i < K; i += 256) reinterpret_cast<__half *>(tp)[i] = __float2half_rn(xval(i));
     } else if (MODE == 1) {
-        const int nsb = K / 256;
-        int8_t * xq = reinterpret_cast<int8_t *>(tp);
-        float * xd = reinterpret_cast<float *>(tp + K);
-        int *   bs = reinterpret_cast<int *>(tp + K + nsb * 4);
-        for (int sb = warp; sb < nsb; sb += 8) {               // quantize_row_q8_K (ggml-quants.c:2768-2805)
-            float v[8]; float amax = 0.0f, mx = 0.0f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { v[j] = xval(sb * 256 + j * 32 + lane); const float av = fabsf(v[j]); if (av > amax) { amax = av; mx = v[j]; } }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float oa = __shfl_xor_sync(0xffffffffu, amax, o), om = __shfl_xor_sync(0xffffffffu, mx, o);
-                if (oa > amax) { amax = oa; mx = om; }
-            }
-            if (amax == 0.0f) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) xq[sb * 256 + j * 32 + lane] = 0;
-                if (lane == 0) xd[sb] = 0.0f;
-                if (lane < 8) bs[sb * 8 + lane] = 0;
-                continue;
-            }
-            const float iscale = -127.0f / mx;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                int q = __float2int_rn(iscale * v[j]); q = min(127, q);
-                xq[sb * 256 + j * 32 + lane] = (int8_t) q;
-                int ssum = q;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
-                if (lane == 0) bs[sb * 8 + j] = ssum;
-            }
-            if (lane == 0) xd[sb] = 1.0f / iscale;
-        }
+        for (int sb = warp; sb < K / 256; sb += 8) q8k_quant_sb(xval, tp, K, sb, lane);
     } else {
         // quantize_row_q8_0 / _q8_1, AVX2 form (ggml-cpu/arch/x86/quants.c): warp per block, lane per element (coalesced)
         for (int b = warp; b < K / 32; b += 8) {
@@ -1145,14 +1104,6 @@ k_gemv_mma(const Gemv2K a) {
             else                  a.v_cache[cell * a.kv_d + (row - 2 * a.kv_d)] = __float2half_rn(v);
         }
     }
-}
-
-size_t act_tok_stride(int wtype, int K) {
-    size_t b;
-    if (wtype == WT_F16) b = (size_t) K * 2;
-    else if (wt_is_kquant(wtype)) b = (size_t) K + (size_t) (K / 256) * 4 + (size_t) (K / 32) * 4;
-    else b = (size_t) K + (size_t) (K / 32) * 4;
-    return (b + 15) & ~size_t(15);
 }
 
 void gemv2(const GemvArgs & a, uint8_t * act_scratch, cudaStream_t st) {

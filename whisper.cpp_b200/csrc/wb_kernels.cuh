@@ -60,9 +60,14 @@ struct GemvArgs {
     // optional KV append (decoder self-attention): rows [kv_d, 2kv_d) -> k_cache, [2kv_d, 3kv_d) -> v_cache, rounded to f16
     __half * k_cache = nullptr; __half * v_cache = nullptr; const int * cells = nullptr; int kv_d = 0;
 };
+// bytes of one token's activation row as both GEMVs hold it (v1: in shared memory, v2: in act_scratch), padded to 16:
+// int8 q[K] | f32 d[K/32] (Q8_0) or {f16 d, f16 s}[K/32] (Q8_1) | f32 d[K/256] + int sum[K/32] (Q8_K); F16 weights: half[K]
+__host__ __device__ inline size_t act_tok_stride(int wtype, int K) {
+    const size_t b = wtype == WT_F16 ? (size_t) K * 2 : (size_t) K + (wt_is_kquant(wtype) ? (size_t) (K / 256) * 4 : 0) + (size_t) (K / 32) * 4;
+    return (b + 15) & ~size_t(15);
+}
 void gemv(const GemvArgs & a, cudaStream_t st);            // v1: dp4a, activation quantisation inside every CTA
-// v2: k_act_quant (one CTA per token) + int8 tensor-core block dots, 32 rows per CTA.  act_scratch: >= 8 * act_tok_stride bytes
-size_t act_tok_stride(int wtype, int K);
+// v2: k_act_quant (one CTA per token) + int8 tensor-core block dots, 16 or 32 rows per CTA.  act_scratch: >= 8 * act_tok_stride bytes
 void gemv2(const GemvArgs & a, uint8_t * act_scratch, cudaStream_t st);
 
 // self-attention for n_tok query tokens over a paged KV cache.  q: [n_tok][d] f32 (already scaled),
