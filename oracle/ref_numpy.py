@@ -87,6 +87,15 @@ def quantize_q8_0(x):
     return q, d.astype(np.float16).astype(np.float32)
 
 
+def q8_0_bytes(x):
+    """block_q8_0 records (ggml-common.h: f16 d, int8 qs[32]) of quantize_q8_0(x)"""
+    q, d = quantize_q8_0(x)
+    out = np.empty((q.shape[0], 34), np.uint8)
+    out[:, 0:2] = d.astype(np.float16).view(np.uint8).reshape(-1, 2)
+    out[:, 2:] = q.astype(np.int8).view(np.uint8)
+    return out.tobytes()
+
+
 def _block_ints(wtype, raw):
     raw = np.frombuffer(raw, dtype=np.uint8)
     bs = {Q4_0: 18, Q5_0: 22, Q8_0: 34}[wtype]

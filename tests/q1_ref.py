@@ -9,8 +9,8 @@ import ctypes as C
 
 import numpy as np
 
-Q4_1, Q5_1, Q8_1 = 3, 7, 9
-BLOCK = {Q4_1: 20, Q5_1: 24, Q8_1: 36}
+Q4_1, Q5_1, Q8_0, Q8_1 = 3, 7, 8, 9
+BLOCK = {Q4_1: 20, Q5_1: 24, Q8_0: 34, Q8_1: 36}
 
 
 def _f16(b):

@@ -11,6 +11,7 @@ import pytest
 from wbtest import (F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K, ref_quantize, bind_whisper_api, read_wav_f32, DATA_DIR,
                     parse_model_header)
 from oracle import ref_numpy as rn
+import kq_signed_ref as kq
 
 pytestmark = pytest.mark.gpu
 vp = C.c_void_p
@@ -86,8 +87,9 @@ def test_gemv_integer_dot_matches_reference_arithmetic(lib, ref, wtype, N, K, n_
 @pytest.mark.parametrize("v2", [0, 4])
 @pytest.mark.parametrize("wtype", [Q4_K, Q5_K])
 def test_gemv_kquants_within_activation_quantisation_noise(lib, ref, wtype, v2):
-    """K-quant GEMV uses Q8_K activations like the reference (ggml-quants.c:2768-2805); checked against exact math
-    with the reference's own int8 noise budget (1e-2 of the output scale)."""
+    """K-quant GEMV uses Q8_K activations like the reference (ggml-quants.c:2768-2805): the reference's Q4_K / Q5_K x Q8_K arithmetic
+    (tests/kq_signed_ref.py, pinned to its vec_dot on the CPU) up to the f32 summation order, 2e-5 of the output scale; and exact math
+    within the reference's own int8 noise budget (1e-2 of the output scale)."""
     rng = np.random.default_rng(5)
     N, K, n_tok = 512, 1280, 2
     w = (rng.standard_normal((N, K)) * 0.05).astype(np.float32)
@@ -100,6 +102,8 @@ def test_gemv_kquants_within_activation_quantisation_noise(lib, ref, wtype, v2):
     assert rc == 0, lib.wb200_last_error()
     want = x.astype(np.float64) @ wd.T
     assert np.abs(out - want).max() < 1e-2 * np.abs(want).max()
+    y = kq.mul_mat_q(wtype, raw, N, K, x)
+    assert np.abs(out - y).max() < 2e-5 * (np.abs(y).max() + 1.0), np.abs(out - y).max()
 
 
 @pytest.mark.parametrize("v2", [0, 4])

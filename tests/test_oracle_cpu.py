@@ -62,6 +62,55 @@ def test_log_mel_float64_restatement_vs_reference(ref):
     ref.whisper_free(ctx)
 
 
+def _q8_0_rows():
+    """Q8_0 activation rows with the quantiser's edges: a zero block, +amax and -amax in one block, a large dynamic range, values on .5
+    boundaries of x * 127 / amax, and ordinary blocks"""
+    rng = np.random.default_rng(3)
+    zero = np.zeros(32, np.float32)
+    tie = rng.uniform(-1, 1, 32).astype(np.float32); tie[3] = 2.0; tie[17] = -2.0
+    wide = (rng.standard_normal(32) * np.float32(10.0) ** rng.integers(-6, 4, 32)).astype(np.float32)
+    half = ((np.arange(32) - 16).astype(np.float32) + np.float32(0.5)) * np.float32(127.0 / 15.5)
+    half[0] = np.float32(127.0)
+    return np.concatenate([zero, tie, wide, half, (rng.standard_normal(32 * 36) * 0.3).astype(np.float32)])
+
+
+@pytest.mark.parametrize("wtype", [Q4_0, Q5_0, Q8_0])
+def test_q8_0_rows_match_reference_bytes(ref, wtype):
+    """rn.quantize_q8_0 writes the bytes of the reference's from_float for the activation type of Q4_0 / Q5_0 / Q8_0 weights"""
+    from q1_ref import RefCpu
+    x = _q8_0_rows()
+    assert rn.q8_0_bytes(x) == RefCpu(ref).quantize_act(wtype, x)
+
+
+@pytest.mark.parametrize("wtype", [Q4_0, Q5_0, Q8_0])
+@pytest.mark.parametrize("K", [384, 1280, 5120])
+def test_q8_0_mul_mat_matches_reference_vec_dot(ref, wtype, K):
+    """rn.mul_mat_q against type_traits_cpu[wtype].vec_dot of the reference's own activation bytes: f32 summation order only, bounded by
+    the recursive-summation bound (blocks + 32 lane partials) * 2^-24 * sum |terms| (the integer sums are exact, so a wrong scale or int
+    moves a result by a whole term)"""
+    from q1_ref import RefCpu
+    cpu = RefCpu(ref)
+    rng = np.random.default_rng(K + wtype)
+    N, n_tok = 24, 3
+    w = (rng.standard_normal((N, K)) * 0.02).astype(np.float32)
+    w[0, :64] = 0.0
+    w[1] *= np.float32(1e3)                                      # an outlier row
+    raw = ref_quantize(ref, wtype, w)
+    x = rng.standard_normal((n_tok, K)).astype(np.float32)
+    x[1, :32] = 0.0
+    x[2] = np.resize(_q8_0_rows(), K)
+    mine = rn.mul_mat_q(wtype, raw, N, K, x)
+    rb = len(raw) // N
+    wi, wd = rn._block_ints(wtype, raw)
+    for t in range(n_tok):
+        xb = cpu.quantize_act(wtype, x[t])
+        xq, xd = rn.quantize_q8_0(x[t])
+        mag = np.abs(np.einsum("nbk,bk->nb", wi.reshape(N, K // 32, 32), xq.reshape(K // 32, 32)) * wd.reshape(N, -1) * xd.reshape(1, -1)).sum(axis=1)
+        for n in range(N):
+            want = cpu.vec_dot(wtype, K, raw[n * rb:(n + 1) * rb], xb)
+            assert abs(mine[t, n] - want) <= (K // 32 + 32) * 2.0 ** -24 * mag[n] + 1e-30, (t, n, mine[t, n], want)
+
+
 def test_q8_0_dot_restatement_matches_exact_math_within_quantisation_noise(ref):
     rng = np.random.default_rng(7)
     w = (rng.standard_normal((64, 256)) * 0.05).astype(np.float32)

@@ -1,5 +1,5 @@
-"""CPU: the NumPy statement of the reference's Q3_K x Q8_K arithmetic (tests/kq_signed_ref.py) against the compiled reference's own
-from_float and vec_dot, and synth's plain Q3_K writer against the reference's dequantize_row_q3_K."""
+"""CPU: the NumPy statement of the reference's Q3_K / Q4_K / Q5_K x Q8_K arithmetic (tests/kq_signed_ref.py) against the compiled
+reference's own from_float and vec_dot, and synth's plain Q3_K writer against the reference's dequantize_row_q3_K."""
 import numpy as np
 import pytest
 
@@ -8,6 +8,7 @@ from wbtest import load_ref, ref_dequantize, ref_quantize
 from e2e_util import synth
 
 WTS = [kq.Q3_K]
+DOT_WTS = [kq.Q3_K, kq.Q4_K, kq.Q5_K]
 
 
 @pytest.fixture(scope="module")
@@ -24,9 +25,14 @@ def _matrix(rng, rows, k):
 
 
 def _extreme_scales(wt, raw, rows):
-    """set the integer scales of row 2 to the extremes of the format (-32 and 31)"""
+    """set the integer scales of row 2 (Q4_K / Q5_K: and row 3) to the extremes of the format: Q3_K -32 and 31; Q4_K / Q5_K 6-bit scales
+    and minimums at 63 / 0 (row 2) and 0 / 63 (row 3)"""
     blk = np.frombuffer(raw, np.uint8).reshape(rows, -1, kq.BLOCK[wt]).copy()
-    blk[2, :, 96:108] = np.array([0x00, 0xFF] * 6, np.uint8)       # stored 0 / 63 patterns: sc - 32 = -32 and 31 mixed
+    if wt == kq.Q3_K:
+        blk[2, :, 96:108] = np.array([0x00, 0xFF] * 6, np.uint8)   # stored 0 / 63 patterns: sc - 32 = -32 and 31 mixed
+    else:                                                          # get_scale_min_k4 of scales[12] = bytes 4 .. 15
+        blk[2, :, 4:16] = np.array([0xFF] * 4 + [0x00] * 4 + [0x0F] * 4, np.uint8)
+        blk[3, :, 4:16] = np.array([0x00] * 4 + [0xFF] * 4 + [0xF0] * 4, np.uint8)
     return blk.tobytes()
 
 
@@ -39,10 +45,11 @@ def test_q8_k_rows_match_reference_bytes(cpu, wt):
     assert kq.q8_k_bytes(x) == cpu.quantize_act(wt, x)
 
 
-@pytest.mark.parametrize("wt", WTS)
+@pytest.mark.parametrize("wt", DOT_WTS)
 @pytest.mark.parametrize("k", [256, 512, 1280, 5120])
 def test_vec_dot_matches_reference(cpu, wt, k):
-    """one dot per row against type_traits_cpu[wt].vec_dot: equal up to the f32 summation order; the integer sumi is exact"""
+    """one dot per row against type_traits_cpu[wt].vec_dot: equal up to the f32 summation order (the integer sums are exact), both the
+    exact statement dot_q8_k and mul_mat_q; the activation rows hold a zero super-block"""
     ref = cpu.ref
     rng = np.random.default_rng(k + wt)
     rows = 6
@@ -50,17 +57,16 @@ def test_vec_dot_matches_reference(cpu, wt, k):
     x = rng.standard_normal((2, k)).astype(np.float32)
     x[1, :256] = 0.0
     got = kq.mul_mat_q(wt, raw, rows, k, x)
-    _, _, wd = kq.block_ints(wt, raw)
-    wd = wd.reshape(rows, k // 256)
     row = kq.BLOCK[wt] * (k // 256)
     for t in range(2):
         xb = cpu.quantize_act(wt, x[t])
         xq, xd = kq.quantize_q8_k(x[t])
-        s = kq.sumi32(wt, raw, rows, k, xq)
-        assert np.abs(s).max() < 2 ** 24                      # the two-k16 combine is exact in f32
-        mag = (np.repeat(np.abs(wd * xd[None, :]), 8, axis=1) * np.abs(s)).sum(axis=1)
+        if wt == kq.Q3_K:
+            assert np.abs(kq.sumi32(wt, raw, rows, k, xq)).max() < 2 ** 24     # the two-k16 combine is exact in f32
+        exact, mag = (v[0] for v in kq.dot_q8_k(wt, raw, rows, k, xq, xd))
         for n in range(rows):
             want = cpu.vec_dot(wt, k, raw[n * row:(n + 1) * row], xb)
+            assert abs(exact[n] - want) <= 1e-6 * mag[n] + 1e-30, (t, n, exact[n], want)
             assert abs(got[t, n] - want) <= 1e-6 * mag[n] + 1e-30, (t, n, got[t, n], want)
 
 

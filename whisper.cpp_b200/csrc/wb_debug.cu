@@ -3,6 +3,7 @@
 #include <cstring>
 #include <vector>
 #include "wb_common.h"
+#include "wb_decode_mk.cuh"
 #include "wb_gemm.cuh"
 #include "wb_kernels.cuh"
 
@@ -239,6 +240,109 @@ int wb200_dbg_planar_dequant(int wtype, int N, int K, const void * w_file, float
     else if (!repack_block32(wtype, wraw.p, planar.p, N, K, &W, 0)) return -4;
     dequant_rows_f32(W, dout.p, 0);
     WB_CUDA_OKV(cudaMemcpy(out, dout.p, (size_t) N * K * 4, cudaMemcpyDeviceToHost), -2);
+    return 0;
+}
+
+// One phase of the persistent decode kernel (mk_probe_launch) from host buffers.  Row buffers have the pass's 64 rows; the phase works on
+// rows [row0, row0 + n_tok) with n_cta CTAs.  `out` is copied to the device before the launch and back after it, so a sentinel fill shows
+// every write.  Per phase (wb_decode_mk.cuh MkProbePhase; actq(K) = the decode kernel's quantised rows of length K, wb_decode_mk.cu):
+//   LNQ:   in = f32 [64][K], bias / scale = LayerNorm b / w [K]            -> out = actq(K)
+//   Q8K:   in = f32 [64][lds]                                              -> out = actq(K)
+//   GEMV:  w_file [N][K], in = actq(K), bias / scale [N], res [64][N], act -> out = f32 [64][N]; with kv_d > 0 outputs [kv_d, 3 kv_d) are
+//          appended as f16 to kc / vc [n_cells][kv_d] (in / out) at cell[64]
+//   GEMV_PAIR (FC1): w_file [N][K], in = actq(K), bias [N]; always GELU   -> out = actq(N)
+//   LOGITS_WARP: w_file [N][K], in = actq(K)                               -> out = f32 [64][N]
+//   ATTN_SELF:  in = f32 qkv rows [64][3d], kc / vc [n_cells][d], nkv [64], idx [64][ld_idx] -> out = actq(d) (K-quants: f32 [64][d])
+//   ATTN_CROSS: in = f32 q rows [64][d], xk / xv head-major [n_slots][n_head][n_keys][64], slot [64] -> out = actq(d) (K-quants: f32 [64][3d],
+//          columns 0 .. d-1 written)
+struct Wb200MkPhaseIo {
+    int wtype, phase, n_cta, row0, n_tok;
+    int N, K, lds, act, kv_d;
+    const void * w_file;
+    const void * in; int64_t in_bytes;
+    const float * bias, * scale, * res;
+    void * out; int64_t out_bytes;
+    const int * cell;
+    uint16_t * kc, * vc; int n_cells;
+    int d, n_head, ld_idx;
+    const int * nkv, * idx;
+    const uint16_t * xk, * xv; int n_keys, n_slots;
+    const int * slot;
+    float kq_scale, eps;
+};
+
+__attribute__((visibility("default")))
+int wb200_dbg_mk_phase(const Wb200MkPhaseIo * io) {
+    constexpr int R = 64;
+    const Wb200MkPhaseIo & s = *io;
+    const bool kq = wt_is_kquant(s.wtype);
+    MkArgs a = {};
+    MkProbe p = {};
+    p.phase = s.phase; p.row0 = s.row0; p.n_tok = s.n_tok; p.act = s.act; p.kv_d = s.kv_d; p.lds = s.lds; p.K = s.K;
+    a.d = s.d; a.n_head = s.n_head; a.n_tok = s.row0 + s.n_tok; a.n_keys = s.n_keys; a.ld_idx = s.ld_idx;
+    a.kq_scale = s.kq_scale; a.eps = s.eps; a.prefetch = 4;     // cross K/V streamed with the evict-first hint, as the engine launches it
+    DevBuf<uint8_t> wraw, tm, din, dout; DevBuf<float> dbias, dscale, dres, dqkv, dq2;
+    DevBuf<int> dcell, dnkv, didx, dslot; DevBuf<__half> dkc, dvc, dxk, dxv; DevBuf<MkLayer> dL; DevBuf<QMat> dW;
+    if (!din.alloc(s.in_bytes) || !dout.alloc(s.out_bytes)) return -1;
+    WB_CUDA_OKV(cudaMemcpy(din.p, s.in, s.in_bytes, cudaMemcpyHostToDevice), -2);
+    WB_CUDA_OKV(cudaMemcpy(dout.p, s.out, s.out_bytes, cudaMemcpyHostToDevice), -2);
+    auto up_f = [&](DevBuf<float> & b, const float * h, size_t n) { if (!h) return true; if (!b.alloc(n)) return false; return cudaMemcpy(b.p, h, n * 4, cudaMemcpyHostToDevice) == cudaSuccess; };
+    auto up_i = [&](DevBuf<int> & b, const int * h, size_t n) { if (!h) return true; if (!b.alloc(n)) return false; return cudaMemcpy(b.p, h, n * 4, cudaMemcpyHostToDevice) == cudaSuccess; };
+    auto up_h = [&](DevBuf<__half> & b, const uint16_t * h, size_t n) { if (!h) return true; if (!b.alloc(n)) return false; return cudaMemcpy(b.p, h, n * 2, cudaMemcpyHostToDevice) == cudaSuccess; };
+    const bool gemv = s.phase == MKP_GEMV || s.phase == MKP_GEMV_PAIR || s.phase == MKP_LOGITS_WARP;
+    if (gemv) {
+        if (wt_tm_rec_bytes(s.wtype) == 0 || s.K % wt_tm_rec_k(s.wtype) || s.K % 32) { set_error("wb200_dbg_mk_phase: no tile-major layout for type %d, K=%d", s.wtype, s.K); return -5; }
+        const size_t wbytes = (size_t) ((double) s.N * s.K * wt_bpw(s.wtype) + 0.5);
+        if (!wraw.alloc(wbytes) || !tm.alloc(wt_tm_bytes(s.wtype, s.N, s.K), true)) return -1;
+        WB_CUDA_OKV(cudaMemcpy(wraw.p, s.w_file, wbytes, cudaMemcpyHostToDevice), -2);
+        p.W.type = s.wtype; p.W.N = s.N; p.W.K = s.K; p.W.base = tm.p; p.W.layout = 1;
+        if (!repack_tile_major(s.wtype, wraw.p, p.W, 0, s.N, 0)) return -4;
+        if (!dW.alloc(1)) return -1;
+        WB_CUDA_OKV(cudaMemcpy(dW.p, &p.W, sizeof(QMat), cudaMemcpyHostToDevice), -2);
+        p.Wg = dW.p;
+        p.x = din.p;
+        if (!up_f(dbias, s.bias, s.N) || !up_f(dscale, s.scale, s.N) || !up_f(dres, s.res, (size_t) R * s.N) || !up_i(dcell, s.cell, R)) return -1;
+        p.bias = dbias.p; p.scale = dscale.p; p.res = dres.p; a.cell = dcell.p;
+        if (s.phase == MKP_GEMV_PAIR) p.dst = dout.p; else p.out = reinterpret_cast<float *>(dout.p);
+        if (s.kv_d > 0) {
+            if (!s.cell || !up_h(dkc, s.kc, (size_t) s.n_cells * s.kv_d) || !up_h(dvc, s.vc, (size_t) s.n_cells * s.kv_d)) return -1;
+            p.kc = dkc.p; p.vc = dvc.p;
+        }
+    } else if (s.phase == MKP_LNQ || s.phase == MKP_Q8K) {
+        p.src = reinterpret_cast<const float *>(din.p); p.dst = dout.p;
+        if (s.phase == MKP_LNQ && (!up_f(dscale, s.scale, s.K) || !up_f(dbias, s.bias, s.K))) return -1;
+        p.scale = dscale.p; p.bias = dbias.p;
+    } else if (s.phase == MKP_ATTN_SELF || s.phase == MKP_ATTN_CROSS) {
+        MkLayer L = {};
+        const bool self = s.phase == MKP_ATTN_SELF;
+        if (!dqkv.alloc((size_t) R * 3 * s.d) || !dq2.alloc((size_t) R * s.d)) return -1;
+        float * const q_in = self ? dqkv.p : dq2.p;
+        WB_CUDA_OKV(cudaMemcpy(q_in, din.p, s.in_bytes, cudaMemcpyDeviceToDevice), -2);
+        if (kq) { if (self) a.q2 = reinterpret_cast<float *>(dout.p); else a.qkv = reinterpret_cast<float *>(dout.p); }
+        else a.actq = dout.p;
+        if (!a.qkv) a.qkv = dqkv.p;
+        if (!a.q2) a.q2 = dq2.p;
+        if (self) {
+            if (!up_h(dkc, s.kc, (size_t) s.n_cells * s.d) || !up_h(dvc, s.vc, (size_t) s.n_cells * s.d) || !up_i(dnkv, s.nkv, R) || !up_i(didx, s.idx, (size_t) R * s.ld_idx)) return -1;
+            L.kc = dkc.p; L.vc = dvc.p; a.nkv = dnkv.p; a.idx = didx.p;
+        } else {
+            const size_t n = (size_t) s.n_slots * s.n_keys * s.d;
+            if (s.n_keys % 128) { set_error("wb200_dbg_mk_phase: n_keys %d is not a multiple of 128", s.n_keys); return -5; }
+            if (!up_h(dxk, s.xk, n) || !up_h(dxv, s.xv, n) || !up_i(dslot, s.slot, R)) return -1;
+            L.xk = dxk.p; L.xv = dxv.p; a.slot = dslot.p; a.slot_stride = (int64_t) s.n_keys * s.d;
+        }
+        if (!dL.alloc(1)) return -1;
+        WB_CUDA_OKV(cudaMemcpy(dL.p, &L, sizeof(L), cudaMemcpyHostToDevice), -2);
+        p.L = dL.p;
+    }
+    if (!mk_probe_launch(a, p, s.wtype, s.n_cta, 0)) return -6;
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { set_error("decode kernel probe: %s", cudaGetErrorString(e)); return -7; }
+    WB_CUDA_OKV(cudaMemcpy(s.out, dout.p, s.out_bytes, cudaMemcpyDeviceToHost), -2);
+    if (s.kc && s.phase == MKP_GEMV && s.kv_d > 0) {
+        WB_CUDA_OKV(cudaMemcpy(s.kc, dkc.p, (size_t) s.n_cells * s.kv_d * 2, cudaMemcpyDeviceToHost), -2);
+        WB_CUDA_OKV(cudaMemcpy(s.vc, dvc.p, (size_t) s.n_cells * s.kv_d * 2, cudaMemcpyDeviceToHost), -2);
+    }
     return 0;
 }
 

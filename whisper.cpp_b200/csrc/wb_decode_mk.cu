@@ -955,6 +955,71 @@ k_decode_pass(const __grid_constant__ MkArgs a) {
     }
 }
 
+// Test probe: one phase, set up as k_decode_pass sets up its CTAs, on a view the caller chooses; no barrier, so an ordinary launch.
+template <int WT, int PHASE>
+__global__ void __launch_bounds__(MK_THREADS, 1)
+k_mk_probe(const __grid_constant__ MkArgs a, const __grid_constant__ MkProbe p) {
+    if (threadIdx.x == 0) { mbar_init(SM_MBAR, 1); SM_FLAG[4] = 0; mbar_fence_init(); }
+    __syncthreads();
+    const MkView v = { (int) blockIdx.x, (int) gridDim.x, p.row0, p.n_tok, 0 };
+    if constexpr (PHASE == MKP_LNQ) mk_lnq<WT>(a, v, p.src, p.K, p.scale, p.bias, p.dst);
+    else if constexpr (PHASE == MKP_Q8K) mk_q8k_rows(v, p.src, p.lds, p.K, p.dst);
+    else if constexpr (PHASE == MKP_GEMV) {
+        MkEpi e;
+        e.bias = p.bias; e.scale = p.scale; e.act = p.act; e.res = p.res; e.out = p.out; e.kc = p.kc; e.vc = p.vc; e.kv_d = p.kv_d;
+        mk_gemv<WT, false>(a, v, p.W, p.x, e);
+    } else if constexpr (PHASE == MKP_GEMV_PAIR) {               // as the pass's FC1 call: epilogue bias + GELU -> rows, matrix in global memory
+        MkEpi e;
+        e.bias = p.bias; e.act = 1; e.qout = p.dst;
+        mk_gemv<WT, true>(a, v, *p.Wg, p.x, e);
+    }
+    else if constexpr (PHASE == MKP_LOGITS_WARP) mk_logits_warp<WT>(a, v, p.W, p.x, p.out);
+    else if constexpr (PHASE == MKP_ATTN_SELF) mk_attn_self<WT>(a, v, *p.L);
+    else mk_attn_cross<WT>(a, v, *p.L);
+}
+
+template <int WT, int PHASE>
+static bool mk_probe_t(const MkArgs & a, const MkProbe & p, int n_cta, cudaStream_t st) {
+    if (ensure_dyn_smem(reinterpret_cast<const void *>(k_mk_probe<WT, PHASE>), MK_SMEM) != cudaSuccess) {
+        set_error("decode kernel probe: cannot raise the shared-memory limit"); return false;
+    }
+    k_mk_probe<WT, PHASE><<<n_cta, MK_THREADS, MK_SMEM, st>>>(a, p);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("decode kernel probe launch: %s", cudaGetErrorString(e)); return false; }
+    return true;
+}
+
+template <int WT>
+static bool mk_probe_w(const MkArgs & a, const MkProbe & p, int n_cta, cudaStream_t st) {
+    switch (p.phase) {
+        case MKP_LNQ:         return mk_probe_t<WT, MKP_LNQ>(a, p, n_cta, st);
+        case MKP_Q8K:         if constexpr (!mk_kq(WT)) break; else return mk_probe_t<WT, MKP_Q8K>(a, p, n_cta, st);
+        case MKP_GEMV:        return mk_probe_t<WT, MKP_GEMV>(a, p, n_cta, st);
+        case MKP_GEMV_PAIR:   if constexpr (mk_kq(WT)) break; else return mk_probe_t<WT, MKP_GEMV_PAIR>(a, p, n_cta, st);   // K-quants: FC1 writes f32 rows
+        case MKP_LOGITS_WARP: return mk_probe_t<WT, MKP_LOGITS_WARP>(a, p, n_cta, st);
+        case MKP_ATTN_SELF:   return mk_probe_t<WT, MKP_ATTN_SELF>(a, p, n_cta, st);
+        case MKP_ATTN_CROSS:  return mk_probe_t<WT, MKP_ATTN_CROSS>(a, p, n_cta, st);
+    }
+    set_error("decode kernel probe: phase %d does not exist for weight type %d", p.phase, WT);
+    return false;
+}
+
+bool mk_probe_launch(const MkArgs & a, const MkProbe & p, int wtype, int n_cta, cudaStream_t st) {
+    if (n_cta < 1 || p.row0 < 0 || p.n_tok < 1 || p.row0 + p.n_tok > MK_MAXTOK) { set_error("decode kernel probe: bad view"); return false; }
+    switch (wtype) {
+        case WT_F16:  return mk_probe_w<WT_F16>(a, p, n_cta, st);
+        case WT_Q4_0: return mk_probe_w<WT_Q4_0>(a, p, n_cta, st);
+        case WT_Q5_0: return mk_probe_w<WT_Q5_0>(a, p, n_cta, st);
+        case WT_Q4_1: return mk_probe_w<WT_Q4_1>(a, p, n_cta, st);
+        case WT_Q5_1: return mk_probe_w<WT_Q5_1>(a, p, n_cta, st);
+        case WT_Q8_0: return mk_probe_w<WT_Q8_0>(a, p, n_cta, st);
+        case WT_Q4_K: return mk_probe_w<WT_Q4_K>(a, p, n_cta, st);
+        case WT_Q5_K: return mk_probe_w<WT_Q5_K>(a, p, n_cta, st);
+        case WT_Q3_K: return mk_probe_w<WT_Q3_K>(a, p, n_cta, st);
+        default: set_error("decode kernel probe: unsupported weight type %d", wtype); return false;
+    }
+}
+
 bool mk_cross_head_major() {
     return true;
 }

@@ -64,4 +64,21 @@ int  mk_max_rows();                 // rows (sequences x tokens) one launch can 
 // cooperative launch on `st`; grid = number of SMs.  Returns false (with the error set) when the launch is refused.
 bool mk_launch(const MkArgs & a, int wtype, int n_sm, cudaStream_t st);
 
+// Test probe (wb200_dbg_mk_phase): ONE phase of the pass run by an ordinary launch of n_cta CTAs on the rows [row0, row0 + n_tok), with
+// the pass's shared-memory carve-up and the same phase functions.  The GEMV phase with the token-embedding matrix is the split-K logits.
+enum MkProbePhase { MKP_LNQ = 0, MKP_Q8K = 1, MKP_GEMV = 2, MKP_GEMV_PAIR = 3, MKP_LOGITS_WARP = 4, MKP_ATTN_SELF = 5, MKP_ATTN_CROSS = 6 };
+struct MkProbe {
+    int phase, row0, n_tok;
+    QMat W;                            // GEMV / logits: tile-major weights
+    const QMat * Wg;                   // the same in device memory (FC1: the pass hands that phase only layer matrices, which live there)
+    const uint8_t * x;                 // GEMV / logits: actq rows (K = W.K)
+    const float * bias, * scale, * res; int act;   // GEMV epilogue (res [64][N]); LN: scale = ln_w, bias = ln_b
+    float * out;                       // GEMV / logits: f32 [64][N]
+    __half * kc, * vc; int kv_d;       // GEMV: K / V append at MkArgs::cell
+    const float * src; int lds, K;     // LN / Q8_K: f32 rows `lds` apart, K values each
+    uint8_t * dst;                     // LN / Q8_K / FC1 PAIR: actq rows
+    const MkLayer * L;                 // attention (device memory, as MkArgs::layers): kc, vc (self), xk, xv (cross)
+};
+bool mk_probe_launch(const MkArgs & a, const MkProbe & p, int wtype, int n_cta, cudaStream_t st);
+
 } // namespace wb
