@@ -254,7 +254,7 @@ int wb200_dbg_planar_dequant(int wtype, int N, int K, const void * w_file, float
 //   LOGITS_WARP: w_file [N][K], in = actq(K)                               -> out = f32 [64][N]
 //   ATTN_SELF:  in = f32 qkv rows [64][3d], kc / vc [n_cells][d], nkv [64], idx [64][ld_idx] -> out = actq(d) (K-quants: f32 [64][d])
 //   ATTN_CROSS: in = f32 q rows [64][d], xk / xv head-major [n_slots][n_head][n_keys][64], slot [64] -> out = actq(d) (K-quants: f32 [64][3d],
-//          columns 0 .. d-1 written)
+//          columns 0 .. d-1 written); N = encoder positions (MkArgs::n_audio_ctx, 0: n_keys): keys N .. n_keys - 1 count as zero rows
 struct Wb200MkPhaseIo {
     int wtype, phase, n_cta, row0, n_tok;
     int N, K, lds, act, kv_d;
@@ -328,6 +328,8 @@ int wb200_dbg_mk_phase(const Wb200MkPhaseIo * io) {
         } else {
             const size_t n = (size_t) s.n_slots * s.n_keys * s.d;
             if (s.n_keys % 128) { set_error("wb200_dbg_mk_phase: n_keys %d is not a multiple of 128", s.n_keys); return -5; }
+            if (s.N < 0 || s.N > s.n_keys) { set_error("wb200_dbg_mk_phase: %d encoder positions for %d keys", s.N, s.n_keys); return -5; }
+            a.n_audio_ctx = s.N > 0 ? s.N : s.n_keys;
             if (!up_h(dxk, s.xk, n) || !up_h(dxv, s.xv, n) || !up_i(dslot, s.slot, R)) return -1;
             L.xk = dxk.p; L.xv = dxv.p; a.slot = dslot.p; a.slot_stride = (int64_t) s.n_keys * s.d;
         }

@@ -593,19 +593,8 @@ __device__ __noinline__ void mk_logits_warp(const MkArgs & a, const MkView v, co
 }
 
 // ---- attention -----------------------------------------------------------------------------------------------------------
-// the 16 query values of this lane's quarter of head h of row t, rounded to f16 (ggml_flash_attn_ext converts Q to f16:
-// ggml-cpu/ops.cpp:8560-8571)
 // Lane quarter r of a key owns dims {8r..8r+7} and {32+8r..32+8r+7} of the head: the 4 lanes of a key then cover 64 contiguous
 // bytes per load instruction (whole 32-byte sectors; 16 dims in a row per lane would use half of every sector it touches).
-__device__ __forceinline__ void load_q16(const float * qh, int r, float (&qv)[16]) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float4 v = __ldcg(reinterpret_cast<const float4 *>(qh + 8 * r + (i >> 1) * 32) + (i & 1));
-        qv[4 * i]     = __half2float(__float2half_rn(v.x)); qv[4 * i + 1] = __half2float(__float2half_rn(v.y));
-        qv[4 * i + 2] = __half2float(__float2half_rn(v.z)); qv[4 * i + 3] = __half2float(__float2half_rn(v.w));
-    }
-}
-
 // One lane owns one key per step: it holds 16 of the 64 dims of that key's K and V rows (the 4 lanes of a key share the score) and
 // keeps its OWN running max / sum / output over the keys it has seen -- no cross-lane traffic per key beyond the 2-step score
 // reduction.  The 8 key slots of a warp are merged once at the end (warp_merge), the warps of a CTA through shared memory.
@@ -688,56 +677,133 @@ __device__ __forceinline__ float attn_merge(const float * pp, int nw, int dim, f
     return o;
 }
 
-// self-attention over the paged cache (whisper.cpp:2603-2625).  Item = (row, head); a pair of warps takes one (8 items per CTA at a time:
-// with 64 rows x 20 heads every item has its warps in the first round).  A lane owns a key quarter; the cells and the K / V pieces of
-// four key groups are requested together, so a row with 200 keys costs a handful of memory round trips instead of one per group.
+// The cp.async ring of the attention phases: MK_RING stages of 64 bytes per thread in the GEMV staging area (idle in these phases).  One
+// stage is one key quarter of a thread, K and V ([k0 | k1 | v0 | v1], 16 bytes each, MK_THREADS * 16 bytes apart); stages are copied
+// MK_RING - 1 ahead of their use.  Every thread reads back only the 64 bytes it copied itself, so the ring needs no barrier -- it is an
+// asynchronous extension of the register file (96 KB in flight per SM; a 6-deep ring was measured slower for the cross stream: the 40 KB of
+// L1 it takes away cost the other phases more than the tail of that phase gains).  cp.async.cg reads through L2 only: K / V rows that other
+// CTAs appended in this pass are seen.
+constexpr int MK_RING = 4, MK_RING_SLOT = MK_THREADS * 64, MK_OFF_QSM = MK_RING * MK_RING_SLOT;
+static_assert(MK_OFF_QSM + 2 * 64 * 4 <= MK_OFF_PART, "the cp.async ring must fit below the attention partials");
+
+__device__ __forceinline__ void cp_wait_ring() { asm volatile("cp.async.wait_group %0;" :: "n"(MK_RING - 1) : "memory"); }
+
+// copy this thread's quarter of K / V row `off` (dims {8r..8r+7}, {32+8r..32+8r+7} of a head) into the ring stage at shared address sa;
+// ef: L2 evict-first
+__device__ __forceinline__ void ring_copy(uint32_t sa, const __half * k, const __half * v, size_t off, bool ef, uint64_t pol) {
+    if (ef) {
+        cp_async16_hint(sa, k + off, pol); cp_async16_hint(sa + MK_THREADS * 16, k + off + 32, pol);
+        cp_async16_hint(sa + 2 * MK_THREADS * 16, v + off, pol); cp_async16_hint(sa + 3 * MK_THREADS * 16, v + off + 32, pol);
+    } else {
+        cp_async16(sa, k + off); cp_async16(sa + MK_THREADS * 16, k + off + 32);
+        cp_async16(sa + 2 * MK_THREADS * 16, v + off); cp_async16(sa + 3 * MK_THREADS * 16, v + off + 32);
+    }
+}
+__device__ __forceinline__ KV4 ring_read(unsigned stage) {
+    const uint8_t * sl = mk_smem + (stage % MK_RING) * MK_RING_SLOT + threadIdx.x * 16;
+    KV4 f;
+    f.k0 = *reinterpret_cast<const uint4 *>(sl);                      f.k1 = *reinterpret_cast<const uint4 *>(sl + MK_THREADS * 16);
+    f.v0 = *reinterpret_cast<const uint4 *>(sl + 2 * MK_THREADS * 16); f.v1 = *reinterpret_cast<const uint4 *>(sl + 3 * MK_THREADS * 16);
+    return f;
+}
+
+// self-attention over the paged cache (whisper.cpp:2603-2625).  Item = (row, head), taken by a pair of warps; the 8 pairs of CTA c take
+// items c*8 + pair, then + 8 nc, ...  Lane (kslot, r) of warp hw of the pair owns key quarter r of the keys 8 hw + 16 i + kslot, i = 0, 1, ..
+// (step i of the warp: 8 keys), and meets them in ascending order.
+// A warp's steps over all its items are ONE stream through the cp.async ring: the loader copies the K / V of a step MK_RING - 1 steps ahead
+// of the arithmetic, across item boundaries, so a warp pays one memory latency per phase, not a chain of them per item.  What the loader
+// needs is fetched ahead too: the cell indices of 16 steps (4 per lane: lane 8s + kslot holds those of steps 4j + s of the batch; a shuffle
+// hands a step's cell to the 4 lanes of its key) for the NEXT batch while the current one is copied; the key counts of the view's rows once
+// per phase (lane i holds rows row0 + i, row0 + 32 + i); the query of the next item while the current one is computed.  Only the first
+// index fetch of the phase is exposed.  An item's result depends on the item alone, never on which pair, CTA or view computes it.
 template <int WT>
 __device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkView v, const MkLayer & L) {
-    constexpr int WPI = 2, SB = 2, CV = 16;                      // warps per item, key groups in flight together (double-buffered), cell indices per lane requested at once
+    constexpr int WPI = 2, NPG = MK_WARPS / WPI;                 // warps per item, warp pairs per CTA
+    static_assert(MK_MAXTOK <= 64, "key counts: two rows per lane");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, grp = warp / WPI, hw = warp % WPI;
-    const int d = a.d, H = a.n_head, n_pairs = v.n_tok * H;
+    const int d = a.d, H = a.n_head, n_items = v.n_tok * H, pstep = v.nc * NPG;
     const int kslot = lane >> 2, r = lane & 3;
-    for (int p = v.ci * (MK_WARPS / WPI) + grp; p < n_pairs; p += v.nc * (MK_WARPS / WPI)) {
-        const int t = v.row0 + p / H, h = p - (t - v.row0) * H;
-        const int nk = a.nkv[t];
-        const int * cells = a.idx + (size_t) t * a.ld_idx;
-        float q[16];
-        load_q16(a.qkv + (size_t) t * 3 * d + h * 64, r, q);
-        LaneAcc A; lane_init(A);
-        // Latency chain of an item: cell indices -> K / V rows -> arithmetic.  The indices of 256 keys (16 per lane) are requested at once,
-        // then the K / V of two key groups at a time, the next two in flight while the current two are used: one round trip for the
-        // indices plus one exposed K / V round trip per item instead of two per 64 keys.  Every lane still meets its keys in ascending order.
-        for (int kb = 0; kb < nk; kb += WPI * 8 * CV) {
-            int cv[CV];
+    int p = v.ci * NPG + grp;                                    // item of the arithmetic
+    if (p >= n_items) return;
+    const int * const idx = a.idx;
+    const int ld_idx = a.ld_idx;
+    // cells of steps 16b .. 16b + 15 of this warp in row t (read up to the end of the index row: the copies check the key count)
+    auto fetch_cells = [&](int (&c)[4], int t, int b) {
+        const int * cells = idx + (size_t) t * ld_idx;
 #pragma unroll
-            for (int i = 0; i < CV; ++i) { const int k = kb + hw * 8 + i * WPI * 8 + kslot; cv[i] = (k < nk) ? __ldg(cells + k) : -1; }
-            KV4 f[2][SB];
-            auto fetch = [&](KV4 (&dst)[SB], int c0, int c1) {
-                const int cc[SB] = { c0, c1 };
+        for (int j = 0; j < 4; ++j) { const int k = 8 * hw + 16 * (16 * b + 4 * j + (lane >> 3)) + (lane & 7); c[j] = (k < ld_idx) ? __ldg(cells + k) : 0; }
+    };
+    int cur[4], nxt[4];                                          // cells of the loader's batch and of the batch after it
+    fetch_cells(nxt, v.row0 + p / H, 0);                         // in flight with the key counts
+    const int nk_lo = lane < v.n_tok ? __ldg(a.nkv + v.row0 + lane) : 0, nk_hi = lane + 32 < v.n_tok ? __ldg(a.nkv + v.row0 + 32 + lane) : 0;
+    auto n_kv = [&](int t) { const int i = t - v.row0; return __shfl_sync(0xffffffffu, i < 32 ? nk_lo : nk_hi, i & 31); };
+    auto n_steps = [&](int nk) { return nk > 8 * hw ? (nk - 8 * hw + 15) >> 4 : 0; };
+    auto seek = [&](int q, int & t, int & h, int & nk, int & ns) {   // the first item >= q with steps for this warp (n_items: none)
+        for (; q < n_items; q += pstep) {
+            t = v.row0 + q / H; h = q - (t - v.row0) * H; nk = n_kv(t); ns = n_steps(nk);
+            if (ns > 0) break;
+        }
+        return q;
+    };
+    // loader: item pl (row tl, head hl, nkl keys, nsl steps), its step il; pn (tn, hn, nkn, nsn): the next item with steps
+    const __half * const kc = L.kc, * const vc = L.vc;
+    const bool ef = (a.prefetch & 4) != 0;
+    const uint64_t pol = policy_evict_first();
+    const uint32_t ring = (uint32_t) __cvta_generic_to_shared(mk_smem) + tid * 16;
+    int tl = 0, hl = 0, nkl = 0, nsl = 0, tn = 0, hn = 0, nkn = 0, nsn = 0, il = 0;
+    int pl = seek(p, tl, hl, nkl, nsl);
+    int pn = pl < n_items ? seek(pl + pstep, tn, hn, nkn, nsn) : n_items;
+    if (pl != p && pl < n_items) fetch_cells(nxt, tl, 0);
+    unsigned is = 0, ic = 0;                                     // stages issued / consumed
+    auto issue = [&]() {                                         // copy the loader's next step (if any) into stage is; always commits a group
+        if (pl < n_items) {
+            const int s = il & 15;
+            if (s == 0) {                                        // a new batch: its cells were requested one batch ago
 #pragma unroll
-                for (int u = 0; u < SB; ++u) {
-                    dst[u].k0 = dst[u].k1 = dst[u].v0 = dst[u].v1 = make_uint4(0, 0, 0, 0);
-                    if (cc[u] >= 0) {
-                        const size_t off = (size_t) cc[u] * d + h * 64 + r * 8;
-                        const uint4 * kp = reinterpret_cast<const uint4 *>(L.kc + off), * vp = reinterpret_cast<const uint4 *>(L.vc + off);
-                        dst[u].k0 = __ldcg(kp); dst[u].k1 = __ldcg(kp + 4); dst[u].v0 = __ldcg(vp); dst[u].v1 = __ldcg(vp + 4);
-                    }
-                }
-            };
-            fetch(f[0], cv[0], cv[1]);
-#pragma unroll
-            for (int g = 0; g < CV / SB; ++g) {
-                const bool more = (g + 1 < CV / SB) && (kb + (g + 1) * SB * WPI * 8 < nk);       // same for both warps of the item
-                if (more) fetch(f[(g + 1) & 1], cv[(2 * g + 2) % CV], cv[(2 * g + 3) % CV]);
-#pragma unroll
-                for (int u = 0; u < SB; ++u) {
-                    float sc = dot16(f[g & 1][u].k0, f[g & 1][u].k1, q);
-                    sc += __shfl_xor_sync(0xffffffffu, sc, 1);
-                    sc += __shfl_xor_sync(0xffffffffu, sc, 2);
-                    if (cv[2 * g + u] >= 0) lane_update(A, sc, f[g & 1][u].v0, f[g & 1][u].v1);
-                }
-                if (!more) break;
+                for (int j = 0; j < 4; ++j) cur[j] = nxt[j];
+                if (il + 16 < nsl) fetch_cells(nxt, tl, (il >> 4) + 1);
+                else if (pn < n_items) fetch_cells(nxt, tn, 0);
             }
+            const int cj = (s >> 2) == 0 ? cur[0] : (s >> 2) == 1 ? cur[1] : (s >> 2) == 2 ? cur[2] : cur[3];
+            const int cell = __shfl_sync(0xffffffffu, cj, (s & 3) * 8 + kslot);
+            if (8 * hw + 16 * il + kslot < nkl) ring_copy(ring + (is % MK_RING) * MK_RING_SLOT, kc, vc, (size_t) cell * d + hl * 64 + r * 8, ef, pol);
+            if (++il == nsl) {
+                il = 0; pl = pn; tl = tn; hl = hn; nkl = nkn; nsl = nsn;
+                if (pl < n_items) pn = seek(pl + pstep, tn, hn, nkn, nsn);
+            }
+        }
+        ++is;
+        cp_commit();
+    };
+#pragma unroll
+    for (int k = 0; k < MK_RING - 1; ++k) issue();
+    const float * const qkv = a.qkv;
+    int t = v.row0 + p / H, h = p - (t - v.row0) * H;
+    float qlo = __ldcg(qkv + (size_t) t * 3 * d + h * 64 + lane), qhi = __ldcg(qkv + (size_t) t * 3 * d + h * 64 + 32 + lane);
+    for (;;) {
+        // the query rounded to f16 (ggml_flash_attn_ext converts Q to f16: ggml-cpu/ops.cpp:8560-8571): q[i] = dim 8r + i, q[8 + i] = dim 32 + 8r + i
+        float q[16];
+        {
+            const float lo = __half2float(__float2half_rn(qlo)), hi = __half2float(__float2half_rn(qhi));
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { q[i] = __shfl_sync(0xffffffffu, lo, 8 * r + i); q[8 + i] = __shfl_sync(0xffffffffu, hi, 8 * r + i); }
+        }
+        const int pq = p + pstep;                                // the next item: its query is requested now
+        int tq = t, hq = h;
+        if (pq < n_items) {
+            tq = v.row0 + pq / H; hq = pq - (tq - v.row0) * H;
+            qlo = __ldcg(qkv + (size_t) tq * 3 * d + hq * 64 + lane); qhi = __ldcg(qkv + (size_t) tq * 3 * d + hq * 64 + 32 + lane);
+        }
+        const int nk = n_kv(t), ns = n_steps(nk);
+        LaneAcc A; lane_init(A);
+        for (int i = 0; i < ns; ++i) {
+            issue();
+            cp_wait_ring();                                      // this thread's copies of stage ic have landed
+            const KV4 f = ring_read(ic++);
+            float sc = dot16(f.k0, f.k1, q);
+            sc += __shfl_xor_sync(0xffffffffu, sc, 1);
+            sc += __shfl_xor_sync(0xffffffffu, sc, 2);
+            if (8 * hw + 16 * i + kslot < nk) lane_update(A, sc, f.v0, f.v1);
         }
         warp_merge(A);
         part_store(SM_PART + (grp * WPI + hw) * MK_PART, A, lane);
@@ -748,24 +814,23 @@ __device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkView v, cons
             mk_store_q<WT>(mk_kq(WT) ? reinterpret_cast<uint8_t *>(a.q2) : a.actq, d, t, h * 64 + hw * 32, lane, (Lsum > 0.0f) ? __fdividef(o, Lsum) : 0.0f);
         }
         bar_named(1 + grp, WPI * 32);
+        if (pq >= n_items) break;
+        p = pq; t = tq; h = hq;
     }
+    cp_wait_all();                                               // the next phase stages its rows over the ring
 }
 
 // cross-attention over the n_keys padded encoder positions, zero rows included (whisper.cpp:2688-2705).
 // K and V of a window live HEAD-MAJOR in HBM ([layer][head][key][64], written that way by the cross GEMM's epilogue): the keys of one
 // (row, head) pair are one contiguous 192 KB stream instead of 128-byte pieces 2.5 KB apart.
 // Work unit = one (row, head) pair over ALL keys; CTA b of the view takes the contiguous range [b*P/G, (b+1)*P/G) of its P pairs.  Warp w, key slot s owns
-// key 8w+s of every 128-key chunk; chunks are copied three ahead with cp.async into a 4-deep ring in shared memory (the GEMV staging
-// area, idle here); every thread reads back only the 64 bytes it copied itself, so the ring needs no barrier -- it is an asynchronous
-// extension of the register file (96 KB in flight per SM; a 6-deep ring was measured slower: the 40 KB of L1 it takes away cost the other
-// phases more than the tail of this one gains).  The arithmetic of a pair (per-lane online softmax over its keys, 8 key slots
-// merged per warp, 16 warps merged per CTA, all in fixed order) never depends on which other rows share the pass: a batch of 64 and a
-// single row give bit-identical results.  (The phase is HBM-bound: a CTA with one pair more than its neighbour is not a cost, the
-// others simply draw more bandwidth meanwhile.)
-constexpr int MK_RING = 4, MK_RING_SLOT = MK_THREADS * 64, MK_OFF_QSM = MK_RING * MK_RING_SLOT;
-static_assert(MK_OFF_QSM + 2 * 64 * 4 <= MK_OFF_PART, "the cp.async ring must fit below the attention partials");
-
-__device__ __forceinline__ void cp_wait_ring() { asm volatile("cp.async.wait_group %0;" :: "n"(MK_RING - 1) : "memory"); }
+// key 8w+s of every 128-key chunk; chunks are copied three ahead with cp.async into the ring.  The arithmetic of a pair (per-lane online
+// softmax over its keys, 8 key slots merged per warp, 16 warps merged per CTA, all in fixed order) never depends on which other rows share
+// the pass: a batch of 64 and a single row give bit-identical results.  (The phase is HBM-bound: a CTA with one pair more than its
+// neighbour is not a cost, the others simply draw more bandwidth meanwhile.)
+// Keys n_audio_ctx .. n_keys - 1 are padding: their K / V rows are zero (the cross K/V buffer is zeroed when it is allocated and whenever
+// the encoded context length changes; the cross GEMM's epilogue writes only the n_audio_ctx real rows).  They stay in the softmax with
+// score 0, as in the reference, but are not read: a thread whose key is padding copies nothing and feeds zero K / V to the same arithmetic.
 
 template <int WT>
 __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, const MkLayer & L) {
@@ -778,7 +843,8 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, con
     unsigned pl = p0, il = 0;
     int jl = 0, tl_ = (int) p0 / H, hl = (int) p0 - tl_ * H;
     const size_t head_stride = (size_t) a.n_keys * 64;
-    const size_t lane_off = (size_t) (warp * 8 + (lane >> 2)) * 64 + (lane & 3) * 8;       // key 8w+s of the chunk, dims {8r.., 32+8r..}
+    const int kw = warp * 8 + (lane >> 2), n_real = a.n_audio_ctx;                        // key 8w+s of the chunk ...
+    const size_t lane_off = (size_t) kw * 64 + (lane & 3) * 8;                              // ... dims {8r.., 32+8r..}
     const uint32_t ring = (uint32_t) __cvta_generic_to_shared(mk_smem) + tid * 16;
     const float kq_scale = a.kq_scale;
     // everything the copy path needs in registers (the asm statements are compiler memory barriers: values re-read from the argument
@@ -793,15 +859,8 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, con
     size_t pair_off = (size_t) slot_cur * slot_stride + (size_t) hl * head_stride + lane_off;
     auto issue = [&]() {                                           // copy the next chunk (if any) into ring slot il % 4; always commits a group
         if (pl < p1) {
-            const size_t off = pair_off + (size_t) (jl * MK_XKEYS) * 64;
-            const uint32_t sa = ring + (il % MK_RING) * MK_RING_SLOT;
-            if (ef) {                                             // L2 evict-first: 500 MB of K / V per layer would otherwise flush the prefetched weights and the activations
-                cp_async16_hint(sa, xk + off, pol); cp_async16_hint(sa + MK_THREADS * 16, xk + off + 32, pol);
-                cp_async16_hint(sa + 2 * MK_THREADS * 16, xv + off, pol); cp_async16_hint(sa + 3 * MK_THREADS * 16, xv + off + 32, pol);
-            } else {
-                cp_async16(sa, xk + off); cp_async16(sa + MK_THREADS * 16, xk + off + 32);
-                cp_async16(sa + 2 * MK_THREADS * 16, xv + off); cp_async16(sa + 3 * MK_THREADS * 16, xv + off + 32);
-            }
+            // L2 evict-first: 500 MB of K / V per layer would otherwise flush the prefetched weights and the activations
+            if (jl * MK_XKEYS + kw < n_real) ring_copy(ring + (il % MK_RING) * MK_RING_SLOT, xk, xv, pair_off + (size_t) (jl * MK_XKEYS) * 64, ef, pol);
             if (++jl == nchp) {
                 jl = 0; ++pl;
                 if (++hl == H) { hl = 0; ++tl_; slot_cur = slot_nxt; slot_nxt = (tl_ + 1 < n_tok) ? slots[tl_ + 1] : 0; }
@@ -824,14 +883,13 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, con
     for (unsigned p = p0; p < p1; ) {
         issue();
         cp_wait_ring();                                          // this thread's copies of chunk ic have landed
-        const uint8_t * sl = mk_smem + (ic % MK_RING) * MK_RING_SLOT + tid * 16;
+        KV4 f = { make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0) };
+        if (j * MK_XKEYS + kw < n_real) f = ring_read(ic);       // padding: the zero row, not read
         ++ic;
-        const uint4 k0 = *reinterpret_cast<const uint4 *>(sl), k1 = *reinterpret_cast<const uint4 *>(sl + MK_THREADS * 16);
-        const uint4 v0 = *reinterpret_cast<const uint4 *>(sl + 2 * MK_THREADS * 16), v1 = *reinterpret_cast<const uint4 *>(sl + 3 * MK_THREADS * 16);
-        float sc = dot16s(k0, k1, qsm + buf * 64 + (lane & 3) * 16);
+        float sc = dot16s(f.k0, f.k1, qsm + buf * 64 + (lane & 3) * 16);
         sc += __shfl_xor_sync(0xffffffffu, sc, 1);
         sc += __shfl_xor_sync(0xffffffffu, sc, 2);
-        lane_update(A, sc * kq_scale, v0, v1);
+        lane_update(A, sc * kq_scale, f.v0, f.v1);
         if (++j < nchp) continue;
         j = 0;                                                   // last chunk of the pair: merge the CTA and write the row's head
         warp_merge(A);
@@ -856,7 +914,7 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, con
         ++p;
         if (++h == H) { h = 0; ++t; }
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");
+    cp_wait_all();
 }
 
 // DTW: copy the alignment-head slices of the cross-Q rows (complete after the barrier that ended phase 6) into the capture buffer

@@ -33,6 +33,7 @@ __host__ __device__ inline MkPart mk_partition(int p, int n_part, int n_cta, int
 struct MkArgs {
     const MkLayer * layers; int n_layer;
     int d, n_head, n_tok, n_keys, ld_idx, n_vocab, want_logits;
+    int n_audio_ctx;                  // encoder positions of the cross K/V (<= n_keys): keys n_audio_ctx .. n_keys - 1 are zero rows
     const int * tok, * pos, * cell, * slot, * nkv, * idx;      // per-row integers of this pass (device)
     int64_t slot_stride;              // elements between the cross KV of consecutive slots
     float kq_scale, eps;

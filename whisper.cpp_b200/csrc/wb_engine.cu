@@ -471,6 +471,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
     if (use_mk) {
         MkArgs a;
         a.layers = mk_layers.p; a.n_layer = Lt; a.d = d; a.n_head = H; a.n_tok = n; a.n_keys = n_keys; a.ld_idx = ld_idx; a.n_vocab = V;
+        a.n_audio_ctx = enc_n_ctx > 0 ? enc_n_ctx : hp.n_audio_ctx;     // n_keys is this rounded up to 256
         a.want_logits = any_logits ? 1 : 0;
         a.tok = d_tok; a.pos = d_pos; a.cell = d_cell; a.slot = d_slot; a.nkv = d_nkv; a.idx = d_idx;
         a.slot_stride = (int64_t) 2 * Lt * Tp * d; a.kq_scale = kq_scale; a.eps = hp.eps;
