@@ -33,7 +33,8 @@ class Io(C.Structure):
                 ("w_file", vp), ("inp", vp), ("in_bytes", C.c_int64), ("bias", vp), ("scale", vp), ("res", vp),
                 ("out", vp), ("out_bytes", C.c_int64), ("cell", vp), ("kc", vp), ("vc", vp), ("n_cells", C.c_int),
                 ("d", C.c_int), ("n_head", C.c_int), ("ld_idx", C.c_int), ("nkv", vp), ("idx", vp),
-                ("xk", vp), ("xv", vp), ("n_keys", C.c_int), ("n_slots", C.c_int), ("slot", vp), ("kq_scale", C.c_float), ("eps", C.c_float)]
+                ("xk", vp), ("xv", vp), ("n_keys", C.c_int), ("n_slots", C.c_int), ("slot", vp), ("kq_scale", C.c_float), ("eps", C.c_float),
+                ("kv_rows", C.c_int)]
 
 
 def _p(a):

@@ -426,48 +426,61 @@ void Group::run(std::vector<Req *> & batch) {
         if (ok && all_samp) ok = eng.set_samp_mask(cfg0->samp->mask_key, *cfg0->samp->mask_bits);
         if (ok && n_cap > 0) ok = eng.dtw_reserve(n_cap);
         if (ok) {
-            std::vector<DecToken> rows; std::vector<int> cells, nkv, idx((size_t) total * ld, 0); std::vector<float *> outs;
             int stride = 1;                                            // entries per row of the sampler output: the widest request decides
             auto own_stride = [](const Req * q) { return (q->samp && q->samp->draws) ? q->samp->stride : 1; };
             if (all_samp) for (Req * q : dec) stride = std::max(stride, own_stride(q));
-            std::vector<int> rowinfo, capidx; std::vector<SampOut> souts((size_t) total * stride); std::vector<std::pair<Req *, int>> origin;
             std::vector<int> cap0(dec.size(), -1);
             for (size_t i = 0, c = 0; i < dec.size(); ++i) if (dec[i]->dtw_n_ctx > 0) { cap0[i] = dtw_req[4 * c]; ++c; }
-            std::vector<double> draws; if (stride > 1) draws.assign((size_t) total * stride, 0.0);
-            rows.reserve(total);
-            // interleave: row k of every request first, so that single-token steps of all members share one pass (<= Engine::max_rows rows)
-            // and multi-token prompts advance in lock-step (causal order inside each member is preserved)
-            int maxn = 0; for (Req * q : dec) maxn = std::max(maxn, q->n);
             for (Req * q : dec) { if (all_samp) { q->st->samp_stride = own_stride(q); q->st->samp_out.assign((size_t) q->n * q->st->samp_stride, SampOut()); } else { q->st->samp_out.clear(); q->st->logits.resize((size_t) q->n * n_vocab); } }
-            for (int k = 0; k < maxn; ++k) {
-                for (size_t i = 0; i < dec.size(); ++i) {
-                    Req * q = dec[i]; if (k >= q->n) continue;
-                    const PreparedDecode & P = preps[i];
-                    const size_t r = rows.size();
-                    rows.push_back(P.rows[k]); cells.push_back(P.cells[k]); nkv.push_back(P.nkv[k]);
-                    memcpy(idx.data() + r * ld, P.idx.data() + (size_t) k * P.ld, (size_t) P.nkv[k] * sizeof(int));
-                    outs.push_back(all_samp ? nullptr : q->st->logits.data() + (size_t) k * n_vocab);
-                    capidx.push_back(cap0[i] >= 0 ? cap0[i] + k : -1);
-                    if (all_samp && q->dtw_n_ctx > 0) {               // DTW row: greedy pick without draws, only its raw summary is read
-                        rowinfo.push_back(0); rowinfo.push_back(0);
-                    } else if (all_samp) {
-                        const bool has_draws = q->samp->draws != nullptr;
-                        rowinfo.push_back(has_draws ? q->samp->rowinfo[2*k] : (q->samp->rowinfo[2*k] & 0xff)); rowinfo.push_back(q->samp->rowinfo[2*k + 1]);
-                        if (has_draws) memcpy(draws.data() + r * stride, q->samp->draws + (size_t) k * q->samp->stride, (size_t) q->samp->stride * sizeof(double));
-                    }
-                    origin.emplace_back(q, k);
-                }
+            // one decode call per encoded context length (a pass attends to one number of cross keys), requests in slot order within each
+            std::vector<std::vector<size_t>> groups; std::vector<int> group_ctx;
+            for (size_t i = 0; i < dec.size(); ++i) {
+                const int T = eng.slot_n_ctx(dec[i]->st->slot);
+                size_t g = 0;
+                while (g < groups.size() && group_ctx[g] != T) ++g;
+                if (g == groups.size()) { groups.emplace_back(); group_ctx.push_back(T); }
+                groups[g].push_back(i);
             }
-            if (all_samp) {
-                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), nullptr, &cfg0->samp->cfg, rowinfo.data(), souts.data(),
-                                stride > 1 ? draws.data() : nullptr, stride, n_cap > 0 ? capidx.data() : nullptr);
-                for (int r = 0; r < total; ++r) {
-                    Req * q = origin[r].first; const int own = own_stride(q);
-                    for (int j = 0; j < own; ++j) q->st->samp_out[(size_t) origin[r].second * own + j] = souts[(size_t) r * stride + j];
+            for (const std::vector<size_t> & grp : groups) {
+                if (!ok) break;
+                int gtotal = 0; for (size_t i : grp) gtotal += dec[i]->n;
+                std::vector<DecToken> rows; std::vector<int> cells, nkv, idx((size_t) gtotal * ld, 0); std::vector<float *> outs;
+                std::vector<int> rowinfo, capidx; std::vector<SampOut> souts((size_t) gtotal * stride); std::vector<std::pair<Req *, int>> origin;
+                std::vector<double> draws; if (stride > 1) draws.assign((size_t) gtotal * stride, 0.0);
+                rows.reserve(gtotal);
+                // interleave: row k of every request first, so that single-token steps of all members share one pass (<= Engine::max_rows rows)
+                // and multi-token prompts advance in lock-step (causal order inside each member is preserved)
+                int maxn = 0; for (size_t i : grp) maxn = std::max(maxn, dec[i]->n);
+                for (int k = 0; k < maxn; ++k) {
+                    for (size_t i : grp) {
+                        Req * q = dec[i]; if (k >= q->n) continue;
+                        const PreparedDecode & P = preps[i];
+                        const size_t r = rows.size();
+                        rows.push_back(P.rows[k]); cells.push_back(P.cells[k]); nkv.push_back(P.nkv[k]);
+                        memcpy(idx.data() + r * ld, P.idx.data() + (size_t) k * P.ld, (size_t) P.nkv[k] * sizeof(int));
+                        outs.push_back(all_samp ? nullptr : q->st->logits.data() + (size_t) k * n_vocab);
+                        capidx.push_back(cap0[i] >= 0 ? cap0[i] + k : -1);
+                        if (all_samp && q->dtw_n_ctx > 0) {               // DTW row: greedy pick without draws, only its raw summary is read
+                            rowinfo.push_back(0); rowinfo.push_back(0);
+                        } else if (all_samp) {
+                            const bool has_draws = q->samp->draws != nullptr;
+                            rowinfo.push_back(has_draws ? q->samp->rowinfo[2*k] : (q->samp->rowinfo[2*k] & 0xff)); rowinfo.push_back(q->samp->rowinfo[2*k + 1]);
+                            if (has_draws) memcpy(draws.data() + r * stride, q->samp->draws + (size_t) k * q->samp->stride, (size_t) q->samp->stride * sizeof(double));
+                        }
+                        origin.emplace_back(q, k);
+                    }
                 }
-            } else {
-                ok = eng.decode(rows.data(), total, cells.data(), idx.data(), ld, nkv.data(), outs.data(), nullptr, nullptr, nullptr, nullptr, 1,
-                                n_cap > 0 ? capidx.data() : nullptr);
+                if (all_samp) {
+                    ok = eng.decode(rows.data(), gtotal, cells.data(), idx.data(), ld, nkv.data(), nullptr, &cfg0->samp->cfg, rowinfo.data(), souts.data(),
+                                    stride > 1 ? draws.data() : nullptr, stride, n_cap > 0 ? capidx.data() : nullptr);
+                    for (int r = 0; r < gtotal; ++r) {
+                        Req * q = origin[r].first; const int own = own_stride(q);
+                        for (int j = 0; j < own; ++j) q->st->samp_out[(size_t) origin[r].second * own + j] = souts[(size_t) r * stride + j];
+                    }
+                } else {
+                    ok = eng.decode(rows.data(), gtotal, cells.data(), idx.data(), ld, nkv.data(), outs.data(), nullptr, nullptr, nullptr, nullptr, 1,
+                                    n_cap > 0 ? capidx.data() : nullptr);
+                }
             }
             // alignment weights of every DTW request of the batch in one launch (the host DTW runs on each state's own thread)
             if (ok && n_cap > 0) {

@@ -253,8 +253,9 @@ int wb200_dbg_planar_dequant(int wtype, int N, int K, const void * w_file, float
 //   GEMV_PAIR (FC1): w_file [N][K], in = actq(K), bias [N]; always GELU   -> out = actq(N)
 //   LOGITS_WARP: w_file [N][K], in = actq(K)                               -> out = f32 [64][N]
 //   ATTN_SELF:  in = f32 qkv rows [64][3d], kc / vc [n_cells][d], nkv [64], idx [64][ld_idx] -> out = actq(d) (K-quants: f32 [64][d])
-//   ATTN_CROSS: in = f32 q rows [64][d], xk / xv head-major [n_slots][n_head][n_keys][64], slot [64] -> out = actq(d) (K-quants: f32 [64][3d],
-//          columns 0 .. d-1 written); N = encoder positions (MkArgs::n_audio_ctx, 0: n_keys): keys N .. n_keys - 1 count as zero rows
+//   ATTN_CROSS: in = f32 q rows [64][d], xk / xv head-major [n_slots][n_head][kv_rows][64], slot [64] -> out = actq(d) (K-quants: f32 [64][3d],
+//          columns 0 .. d-1 written); N = encoder positions (MkArgs::n_audio_ctx, 0: n_keys): keys N .. n_keys - 1 count as zero rows;
+//          kv_rows = rows per head of the buffer (MkArgs::kv_rows, 0: n_keys), the engine's is its largest padded context
 struct Wb200MkPhaseIo {
     int wtype, phase, n_cta, row0, n_tok;
     int N, K, lds, act, kv_d;
@@ -269,6 +270,7 @@ struct Wb200MkPhaseIo {
     const uint16_t * xk, * xv; int n_keys, n_slots;
     const int * slot;
     float kq_scale, eps;
+    int kv_rows;
 };
 
 __attribute__((visibility("default")))
@@ -326,12 +328,14 @@ int wb200_dbg_mk_phase(const Wb200MkPhaseIo * io) {
             if (!up_h(dkc, s.kc, (size_t) s.n_cells * s.d) || !up_h(dvc, s.vc, (size_t) s.n_cells * s.d) || !up_i(dnkv, s.nkv, R) || !up_i(didx, s.idx, (size_t) R * s.ld_idx)) return -1;
             L.kc = dkc.p; L.vc = dvc.p; a.nkv = dnkv.p; a.idx = didx.p;
         } else {
-            const size_t n = (size_t) s.n_slots * s.n_keys * s.d;
+            const int rows = s.kv_rows > 0 ? s.kv_rows : s.n_keys;
+            const size_t n = (size_t) s.n_slots * rows * s.d;
             if (s.n_keys % 128) { set_error("wb200_dbg_mk_phase: n_keys %d is not a multiple of 128", s.n_keys); return -5; }
             if (s.N < 0 || s.N > s.n_keys) { set_error("wb200_dbg_mk_phase: %d encoder positions for %d keys", s.N, s.n_keys); return -5; }
-            a.n_audio_ctx = s.N > 0 ? s.N : s.n_keys;
+            if (rows < s.n_keys) { set_error("wb200_dbg_mk_phase: %d rows per head for %d keys", rows, s.n_keys); return -5; }
+            a.n_audio_ctx = s.N > 0 ? s.N : s.n_keys; a.kv_rows = rows;
             if (!up_h(dxk, s.xk, n) || !up_h(dxv, s.xv, n) || !up_i(dslot, s.slot, R)) return -1;
-            L.xk = dxk.p; L.xv = dxv.p; a.slot = dslot.p; a.slot_stride = (int64_t) s.n_keys * s.d;
+            L.xk = dxk.p; L.xv = dxv.p; a.slot = dslot.p; a.slot_stride = (int64_t) rows * s.d;
         }
         if (!dL.alloc(1)) return -1;
         WB_CUDA_OKV(cudaMemcpy(dL.p, &L, sizeof(L), cudaMemcpyHostToDevice), -2);

@@ -821,15 +821,17 @@ __device__ __noinline__ void mk_attn_self(const MkArgs & a, const MkView v, cons
 }
 
 // cross-attention over the n_keys padded encoder positions, zero rows included (whisper.cpp:2688-2705).
-// K and V of a window live HEAD-MAJOR in HBM ([layer][head][key][64], written that way by the cross GEMM's epilogue): the keys of one
-// (row, head) pair are one contiguous 192 KB stream instead of 128-byte pieces 2.5 KB apart.
+// K and V of a window live HEAD-MAJOR in HBM ([layer][head][kv_rows][64], written that way by the cross GEMM's epilogue with kv_rows =
+// the engine's largest padded context): the keys of one (row, head) pair are one contiguous 192 KB stream instead of 128-byte pieces
+// 2.5 KB apart.  A reduced context reads the first n_keys rows of each head's kv_rows.
 // Work unit = one (row, head) pair over ALL keys; CTA b of the view takes the contiguous range [b*P/G, (b+1)*P/G) of its P pairs.  Warp w, key slot s owns
 // key 8w+s of every 128-key chunk; chunks are copied three ahead with cp.async into the ring.  The arithmetic of a pair (per-lane online
 // softmax over its keys, 8 key slots merged per warp, 16 warps merged per CTA, all in fixed order) never depends on which other rows share
 // the pass: a batch of 64 and a single row give bit-identical results.  (The phase is HBM-bound: a CTA with one pair more than its
 // neighbour is not a cost, the others simply draw more bandwidth meanwhile.)
-// Keys n_audio_ctx .. n_keys - 1 are padding: their K / V rows are zero (the cross K/V buffer is zeroed when it is allocated and whenever
-// the encoded context length changes; the cross GEMM's epilogue writes only the n_audio_ctx real rows).  They stay in the softmax with
+// Keys n_audio_ctx .. n_keys - 1 are padding: their K / V rows are zero (the cross K/V buffer is zeroed when it is allocated, and an
+// encode at a reduced context zeroes the rows past it in the slots it writes; the cross GEMM's epilogue writes only the n_audio_ctx real
+// rows).  They stay in the softmax with
 // score 0, as in the reference, but are not read: a thread whose key is padding copies nothing and feeds zero K / V to the same arithmetic.
 
 template <int WT>
@@ -842,7 +844,7 @@ __device__ __noinline__ void mk_attn_cross(const MkArgs & a, const MkView v, con
     // loader state: chunk being fetched
     unsigned pl = p0, il = 0;
     int jl = 0, tl_ = (int) p0 / H, hl = (int) p0 - tl_ * H;
-    const size_t head_stride = (size_t) a.n_keys * 64;
+    const size_t head_stride = (size_t) a.kv_rows * 64;                                   // head h of a layer starts at h * kv_rows * 64
     const int kw = warp * 8 + (lane >> 2), n_real = a.n_audio_ctx;                        // key 8w+s of the chunk ...
     const size_t lane_off = (size_t) kw * 64 + (lane & 3) * 8;                              // ... dims {8r.., 32+8r..}
     const uint32_t ring = (uint32_t) __cvta_generic_to_shared(mk_smem) + tid * 16;

@@ -34,6 +34,7 @@ struct MkArgs {
     const MkLayer * layers; int n_layer;
     int d, n_head, n_tok, n_keys, ld_idx, n_vocab, want_logits;
     int n_audio_ctx;                  // encoder positions of the cross K/V (<= n_keys): keys n_audio_ctx .. n_keys - 1 are zero rows
+    int kv_rows;                      // rows per head of the cross K/V buffer (>= n_keys): the producer's layout, not the pass's key count
     const int * tok, * pos, * cell, * slot, * nkv, * idx;      // per-row integers of this pass (device)
     int64_t slot_stride;              // elements between the cross KV of consecutive slots
     float kq_scale, eps;

@@ -58,6 +58,7 @@ bool Engine::init(const Model * model, int cap_windows) {
     gemv_v2 = getenv("WB200_GEMV_V1") == nullptr;
     (void) B; (void) H; (void) M; (void) Tp;
     if (!alloc_encoder_ws() || !kv_cross.alloc((size_t) cap_win * 2 * Lt * Tp * d, true)) return false;
+    slot_ctx.assign((size_t) cap_win, 0);
     {
         cudaDeviceProp prop; WB_CUDA_OK(cudaGetDeviceProperties(&prop, m->device));
         n_sm = prop.multiProcessorCount;
@@ -118,6 +119,7 @@ bool Engine::resize(int new_cap, int new_cps) {
         if (!nx.alloc((size_t) new_cap * slot_e, true)) return false;
         if (kv_cross.p) WB_CUDA_OK(cudaMemcpy(nx.p, kv_cross.p, (size_t) keep * slot_e * sizeof(__half), cudaMemcpyDeviceToDevice));
         std::swap(nx.p, kv_cross.p); std::swap(nx.n, kv_cross.n);
+        slot_ctx.resize((size_t) new_cap, 0);                     // the context length of each surviving slot's cross K/V goes with it
     }
     if (new_cap != old_cap || new_cps != old_cps || !kv_k.p) {
         const size_t e = (size_t) Lt * new_cap * new_cps * d;
@@ -381,8 +383,7 @@ bool Engine::encode(const EncSrc * srcs, int n_win, int n_ctx) {
     if (n_win < 1 || n_win > cap_win) { set_error("encode: n_win=%d exceeds the state's capacity %d", n_win, cap_win); return false; }
     if (n_ctx <= 0 || n_ctx > hp.n_audio_ctx) { set_error("encode: bad n_ctx %d", n_ctx); return false; }
     if (!plan || plan->n_ctx != n_ctx || plan->n_win != n_win) {
-        if (plan && plan->n_ctx != n_ctx) {   // different padding: make sure padded key rows are zero again
-            WB_CUDA_OK(cudaMemsetAsync(kv_cross.p, 0, kv_cross.bytes(), st));
+        if (plan && plan->n_ctx != n_ctx) {   // different padding: make sure the encoder's padded key rows are zero again
             WB_CUDA_OK(cudaMemsetAsync(vt.p, 0, vt.bytes(), st));
             WB_CUDA_OK(cudaMemsetAsync(h1.p, 0, h1.bytes(), st));
         }
@@ -424,6 +425,18 @@ bool Engine::encode(const EncSrc * srcs, int n_win, int n_ctx) {
     }
     layernorm(x.p, m->e_ln.w, m->e_ln.b, hp.eps, NT, d, enc16.p, debug_taps ? enc32.p : nullptr, st);
     WB_CUDA_OK(cudaEventRecord(ev[3], st));
+    if (T < hp.n_audio_ctx) {
+        // The cross GEMM writes rows [0, T) of each head (head-major) or block (token-major); rows [T, Tp_max) of the slots written here
+        // may hold an earlier, longer encode and must read as zero keys: both decoders attend to the padding up to pad256(T).  Rows from
+        // n_audio_ctx on are never written, so a full-context encode has nothing to clear.  Other slots keep their cross K/V untouched.
+        const int dt = hp.n_text_state, Lt = hp.n_text_layer;
+        const bool hm = use_mk && mk_cross_head_major();
+        const size_t row = hm ? 64 : (size_t) dt, blocks = hm ? (size_t) 2 * Lt * (dt / 64) : (size_t) 2 * Lt;
+        for (int w = 0; w < n_win; ++w) {
+            __half * base = kv_cross.p + (size_t) srcs[w].slot * 2 * Lt * Tp_max * dt;
+            WB_CUDA_OK(cudaMemset2DAsync(base + (size_t) T * row, (size_t) Tp_max * row * sizeof(__half), 0, (size_t) (Tp_max - T) * row * sizeof(__half), blocks, st));
+        }
+    }
     if (identity_slots) {
         WB_GEMM(PL.cross);
     } else {                          // windows land in arbitrary cross-KV slots: one launch per window
@@ -441,6 +454,7 @@ bool Engine::encode(const EncSrc * srcs, int n_win, int n_ctx) {
     cudaEventElapsedTime(&last_ms[3], ev[3], ev[4]);
     counter_add(4, 1); counter_add(5, n_win); counter_add(6, last_ms[1] + last_ms[2] + last_ms[3]);
     enc_n_ctx = n_ctx; enc_n_win = n_win;
+    for (int w = 0; w < n_win; ++w) slot_ctx[(size_t) srcs[w].slot] = n_ctx;
     return true;
 }
 
@@ -455,7 +469,7 @@ bool Engine::set_samp_mask(uint64_t key, const std::vector<uint32_t> & bits) {
     return true;
 }
 
-bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampCfg * samp) {
+bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp) {
     const HParams & hp = m->hp;
     const int d = hp.n_text_state, H = hp.n_text_head, Lt = hp.n_text_layer, V = hp.n_vocab;
     const int Tp = Tp_max;                                         // kv_cross layout stride
@@ -471,7 +485,8 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampC
     if (use_mk) {
         MkArgs a;
         a.layers = mk_layers.p; a.n_layer = Lt; a.d = d; a.n_head = H; a.n_tok = n; a.n_keys = n_keys; a.ld_idx = ld_idx; a.n_vocab = V;
-        a.n_audio_ctx = enc_n_ctx > 0 ? enc_n_ctx : hp.n_audio_ctx;     // n_keys is this rounded up to 256
+        a.n_audio_ctx = n_audio_ctx;                                    // n_keys is this rounded up to 256
+        a.kv_rows = Tp;                                                 // the cross GEMM lays each head out over Tp_max rows
         a.want_logits = any_logits ? 1 : 0;
         a.tok = d_tok; a.pos = d_pos; a.cell = d_cell; a.slot = d_slot; a.nkv = d_nkv; a.idx = d_idx;
         a.slot_stride = (int64_t) 2 * Lt * Tp * d; a.kq_scale = kq_scale; a.eps = hp.eps;
@@ -558,7 +573,6 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
     const HParams & hp = m->hp;
     WB_CUDA_OK(cudaSetDevice(m->device));
     const int V = hp.n_vocab;
-    const int n_keys = pad256(enc_n_ctx > 0 ? enc_n_ctx : hp.n_audio_ctx);
 
     const int64_t t_host0 = std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
     const int R = max_rows;
@@ -582,6 +596,11 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
             pass_capture |= h_cap[j] >= 0;
             any_logits |= t.want_logits;
         }
+        const int n_ctx = slot_n_ctx(rows[r0].slot), n_keys = pad256(n_ctx);   // encoder positions of the pass's cross K/V
+        for (int j = 1; j < n; ++j)
+            if (slot_n_ctx(rows[r0 + j].slot) != n_ctx) {
+                set_error("decode: one pass over slots encoded at %d and %d positions", n_ctx, slot_n_ctx(rows[r0 + j].slot)); return false;
+            }
         draw_stride = (samp && draws && stride > 1) ? std::min(stride, (int) SAMP_MAX_DRAWS) : 1;
         if (draw_stride > 1) {
             for (int j = 0; j < n; ++j) memcpy(hdraws + (size_t) j * draw_stride, draws + (size_t) (r0 + j) * stride, (size_t) draw_stride * sizeof(double));
@@ -607,7 +626,7 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
             const uint64_t l0 = launch_count();
             cudaGraph_t g = nullptr;
             WB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const bool ok = decode_pass_enqueue(n, any_logits, n_keys, samp);
+            const bool ok = decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp);
             const cudaError_t ce = cudaStreamEndCapture(st, &g);
             if (!ok || ce != cudaSuccess) { if (g) cudaGraphDestroy(g); set_error("decode: graph capture failed: %s", cudaGetErrorString(ce)); return false; }
             sg->launches = launch_count() - l0;
@@ -617,7 +636,7 @@ bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const 
             WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
         } else {
             if (sg) sg->seen++;
-            if (!decode_pass_enqueue(n, any_logits, n_keys, samp)) return false;
+            if (!decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp)) return false;
         }
         WB_CUDA_OK(cudaEventRecord(ev[6], st));
         WB_CUDA_OK(cudaStreamSynchronize(st));

@@ -59,6 +59,8 @@ struct Engine {
     bool gemm_v2 = true;             // WB200_GEMM_V1=1 selects the first-generation kernel (in-kernel dequantisation, one tile per CTA)
     DevBuf<__half> kv_cross;         // [cap_win][2][Lt][Tp][d]; with the persistent decode kernel (use_mk) each [Tp][d] block is head-major [d/64][Tp][64]
     int enc_n_ctx = 0, enc_n_win = 0;   // what the last encode produced
+    std::vector<int> slot_ctx;       // per cross-KV slot: encoder positions of its last encode (0: never encoded); states of one pool may differ
+    int slot_n_ctx(int slot) const { return slot_ctx[(size_t) slot] > 0 ? slot_ctx[(size_t) slot] : m->hp.n_audio_ctx; }
     EncPlan * plan = nullptr;
 
     // ---- decoder
@@ -128,7 +130,9 @@ struct Engine {
 
     // decode a batch (<= max_rows rows per pass internally).  idx lists: for row j, cells[j] is where its K/V go and
     // (kv_idx[j*ld .. +n_kv[j]]) the cells it attends to.  logits_out[j]: host buffer of n_vocab floats for rows with want_logits.
-    bool decode_pass_enqueue(int n, bool any_logits, int n_keys, const SampCfg * samp);   // the kernels of one pass (<= max_rows rows) on `st`
+    // The slots of the rows of one pass must hold cross K/V of the same context length (slot_n_ctx); a pass that mixes them is an error.
+    // the kernels of one pass (<= max_rows rows) on `st`; every row's slot holds cross K/V of n_audio_ctx positions, n_keys = pad256 of it
+    bool decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp);
     // samp != nullptr: logits stay on the device; the filter + greedy pick run there (rowinfo: 2 ints per row, samp_out: host [n_rows])
     bool decode(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, float * const * logits_out,
                 const SampCfg * samp = nullptr, const int * rowinfo = nullptr, SampOut * samp_out = nullptr,
