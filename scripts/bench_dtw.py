@@ -4,9 +4,10 @@ whisper_full_parallel(ctx, params, pcm, n, n) -- the bench.py default workload (
 dtw_token_timestamps on (alignment heads: preset large-v3) or off.
 
 One process measures one build (the library named by WB200_LIB, else the in-tree one); to compare builds, run the script once per build,
-alternating, and compare the JSON lines.  Reported: x real time, decode passes and rows, the alignment-weight kernel's GPU time, the host
-DTW time (summed over the member threads), and the device->host bytes (wb200_traffic) -- with DTW on they should exceed DTW off by the
-alignment-weight copies alone.  Counters a build does not have (k_dtw_qk time and host DTW time before they existed) read as 0.
+alternating, and compare the JSON lines.  Reported: x real time, decode passes and rows, the alignment-weight kernel's GPU time, the
+device DTW path kernels' GPU time, the host DTW time (summed over the member threads), and the device->host bytes (wb200_traffic) -- with
+DTW on they should exceed DTW off by the alignment-weight copies and the paths alone.  Counters a build does not have (k_dtw_qk time, host
+DTW time, device DTW path time before they existed) read as 0.
 
   python scripts/bench_dtw.py --dtw on|off [--chunks 64] [--warmup 1] [--tag NAME]
 """
@@ -86,7 +87,7 @@ def main():
     out = {"tag": args.tag, "lib": os.path.basename(os.path.dirname(pkg.LIB_PATH)) + "/" + os.path.basename(pkg.LIB_PATH), "dtw": args.dtw, "chunks": n,
            "audio_s": len(pcm) / 16000.0, "wall_s": round(dt, 3), "xRT": round(len(pcm) / 16000.0 / dt, 1), "tokens": n_tok, "tokens_with_t_dtw": dtw_set,
            "decode_passes": int(d[0]), "decode_rows": int(d[1]), "decode_gpu_ms": round(d[2], 1), "encode_windows": int(d[5]),
-           "dtw_qk_gpu_ms": round(d[8], 2), "dtw_passes": int(d[9]), "host_dtw_ms": round(d[10], 1), "h2d_bytes": int(d[16]), "d2h_bytes": int(d[17]),
+           "dtw_qk_gpu_ms": round(d[8], 2), "dtw_passes": int(d[9]), "dtw_path_gpu_ms": round(d[11], 2), "host_dtw_ms": round(d[10], 1), "h2d_bytes": int(d[16]), "d2h_bytes": int(d[17]),
            "card": card()}
     print(json.dumps(out), flush=True)
     L.whisper_free(ctx)

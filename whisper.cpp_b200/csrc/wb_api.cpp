@@ -171,14 +171,14 @@ bool encode_window(whisper_context & ctx, whisper_state & st, int mel_offset) {
 }
 
 bool decode_batch(whisper_context & ctx, whisper_state & st, const int * tokens, const int * pos, const int * seq,
-                  const int8_t * want, int n_tokens, const SampReq * samp, int dtw_n_ctx) {
+                  const int8_t * want, int n_tokens, const SampReq * samp, int dtw_n_ctx, int dtw_sot_len, int dtw_n_frames) {
     if (st.scripted) {                                                       // test hook: what was fed to the decoder (wb200_dbg_last_batch)
         st.dbg_tok.assign(tokens, tokens + n_tokens); st.dbg_pos.assign(pos, pos + n_tokens);
         st.dbg_seq.assign(seq, seq + n_tokens); st.dbg_want.assign(want, want + n_tokens);
     }
     if (!st.group) { set_error("decode: the state is not attached to a device pool"); return false; }
     Group::Req r; r.kind = 1; r.ctx = &ctx; r.st = &st; r.tokens = tokens; r.pos = pos; r.seq = seq; r.want = want; r.n = n_tokens; r.samp = samp;
-    r.dtw_n_ctx = dtw_n_ctx;
+    r.dtw_n_ctx = dtw_n_ctx; r.dtw_sot_len = dtw_sot_len; r.dtw_n_frames = dtw_n_frames;
     if (!st.group->submit(r)) return false;
     account_decode(st, n_tokens, r.dt_us);
     note_rows(ctx, st, want, n_tokens);
@@ -410,10 +410,11 @@ void Group::run(std::vector<Req *> & batch) {
         };
         for (Req * q : dec) if (!q->dtw_n_ctx) all_samp = all_samp && q->samp != nullptr && q->samp->mask_key == cfg0->samp->mask_key && same_cfg(q->samp->cfg, cfg0->samp->cfg);
         // DTW requests: capture indices [cap0, cap0 + n) of the engine's capture buffer, one region per request
-        std::vector<int> dtw_req; std::vector<Req *> dtw_of;
+        std::vector<int> dtw_req, dtw_path; std::vector<Req *> dtw_of;
         int n_cap = 0;
         for (Req * q : dec) if (q->dtw_n_ctx > 0) {
             dtw_req.insert(dtw_req.end(), { n_cap, q->st->slot, q->n, q->dtw_n_ctx });
+            dtw_path.insert(dtw_path.end(), { q->dtw_n_frames / 2, q->dtw_sot_len });
             dtw_of.push_back(q); n_cap += q->n;
         }
         if (scripted) {                                               // test hook: KV bookkeeping done above, logits are the callback's business
@@ -482,11 +483,12 @@ void Group::run(std::vector<Req *> & batch) {
                                     n_cap > 0 ? capidx.data() : nullptr);
                 }
             }
-            // alignment weights of every DTW request of the batch in one launch (the host DTW runs on each state's own thread)
+            // alignment weights and warping paths of every DTW request of the batch, one launch per kernel (dtw_assign runs on each state's
+            // own thread)
             if (ok && n_cap > 0) {
-                std::vector<std::vector<float> *> outw;
-                for (Req * q : dtw_of) outw.push_back(&q->st->dtw_qk_last);
-                ok = eng.dtw_weights(dtw_req, outw);
+                std::vector<std::vector<float> *> outw; std::vector<std::vector<int32_t> *> outt, outj;
+                for (Req * q : dtw_of) { outw.push_back(&q->st->dtw_qk_last); outt.push_back(&q->st->dtw_tok); outj.push_back(&q->st->dtw_time); }
+                ok = eng.dtw_weights(dtw_req, dtw_path, outw, outt, outj);
                 for (Req * q : dtw_of) { whisper_state & s = *q->st; s.dtw_last_shape[0] = q->n; s.dtw_last_shape[1] = q->dtw_n_ctx; s.dtw_last_shape[2] = eng.dtw_n_heads; }
             }
         }
@@ -1012,6 +1014,13 @@ WB_EXPORT int wb200_dbg_last_attended(struct whisper_state * st, uint64_t * out,
     if (!st || !st->scripted || (int) st->dbg_att.size() > cap) return -1;
     for (size_t i = 0; i < st->dbg_att.size(); ++i) out[i] = st->dbg_att[i];
     return (int) st->dbg_att.size();
+}
+
+// test hook: the window of the last DTW pass of this state: {mel frames, sot_len, seek, DTW passes of the state so far}
+WB_EXPORT int wb200_dbg_last_dtw_window(struct whisper_state * st, int * out) {
+    if (!st || !out) return -1;
+    for (int i = 0; i < 4; ++i) out[i] = st->dtw_last_window[i];
+    return 0;
 }
 
 // test hook: alignment-head weights of the last DTW pass of this state [heads][n_audio_ctx][tokens]; shape = {tokens, n_audio_ctx, heads}

@@ -1,7 +1,8 @@
 // wb_dtw.h -- DTW token timestamps (whisper_context_params.dtw_token_timestamps; src/whisper.cpp:8856-9167).
 // The cross-attention weights of the alignment heads come from the device (one extra decoder pass over the window's text, batched with the
-// other states of the pool, whose rows capture the alignment-head queries; k_dtw_qk); everything after that -- normalisation over the tokens, 7-tap median filter over time, mean over
-// heads, dynamic time warping, backtrace, assignment to tokens -- is host code here.
+// other states of the pool, whose rows capture the alignment-head queries; k_dtw_qk), and so does the warping path (normalisation over
+// the tokens, 7-tap median filter over time, mean over heads, dynamic time warping, backtrace; DtwPaths, wb_dtw_kernel.cuh).  dtw_path
+// below is the host reference those kernels reproduce bit for bit; the assignment of the path to the tokens (dtw_assign) is host code.
 #pragma once
 #include <cstdint>
 #include <utility>

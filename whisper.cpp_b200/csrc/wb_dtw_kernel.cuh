@@ -10,6 +10,8 @@
 #include <cstdint>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <vector>
+#include "wb_common.h"
 
 namespace wb {
 
@@ -33,6 +35,37 @@ struct DtwQkArgs {
 bool dtw_qk_launch(const DtwQkArgs & a, cudaStream_t st);
 // the same phases walked on the host (test hook; pointers are host pointers)
 void dtw_qk_emulated(const DtwQkArgs & a);
+
+// ---- the warping path of each request, computed from its weights on the device (dtw_path of wb_dtw.cpp, bit for bit)
+// Per request: 5 ints (n_tokens, n_audio_ctx, n_heads, M = audio positions used, sot_len); N = n_tokens - sot_len - 1 path rows.
+// Three launches cover every request of a batch: k_dtw_norm (mean and scale of each (head, position) column over the tokens),
+// k_dtw_cost (7-wide median over time per head, mean over heads, negated: cost [N][M]) and k_dtw_sweep (one CTA per request: anti-diagonal
+// sweep with 2-bit trace codes in shared memory, then the backtrace).  Every f32 operation the host does separately is an _rn intrinsic
+// on the device (nvcc would contract a*b + c into an FMA) and a plain operator in the host walk; double sums keep the host's order.
+// A request with N <= 0, M <= 7 or no heads gets an empty path, like dtw_path.
+constexpr int DTW_REQ_INTS = 5;
+struct DtwPathArgs {
+    const float * w;             // weights: request r at w + off[4r], [n_heads][n_audio_ctx][n_tokens]
+    const int * req;             // DTW_REQ_INTS per request
+    const int64_t * off;         // per request, 4 offsets: weights (floats of w), column stats (float2 of stat), cost (floats), path (ints)
+    float2 * stat;               // [n_heads][M] (mean, scale) per request
+    float * cost;                // [N][M] per request
+    int * path;                  // per request: tok_idx [N + M], time_idx [N + M], then the path length (1 int)
+    int n_req;
+};
+
+// grow-only device buffers of a batch of path requests
+class DtwPaths {
+  public:
+    // upload req / weight offsets (request r's weights at w + w_off[r], device memory) and launch the three kernels on st
+    bool enqueue(const float * w, const std::vector<int> & req, const std::vector<int64_t> & w_off, cudaStream_t st);
+    bool fetch(cudaStream_t st);      // queue the copy of every path to the host
+    // after st has synchronised: the path of request r (tok_idx, time_idx in path order)
+    void get(int r, std::vector<int32_t> & tok, std::vector<int32_t> & time) const;
+  private:
+    DevBuf<int> d_req, d_path; DevBuf<int64_t> d_off; DevBuf<float2> d_stat; DevBuf<float> d_cost;
+    std::vector<int> h_req, h_path; std::vector<int64_t> h_off;
+};
 
 // chain path: copy the alignment-head slices of the rows of one pass from the cross-Q output q [n_rows][d]
 bool dtw_capture_launch(const float * q, int d, const int * cap_row, int n_rows, uint32_t head_mask, int cap_head0, float * cap, int cap_rows, cudaStream_t st);

@@ -694,7 +694,8 @@ bool Engine::dtw_reserve(int n_rows) {
     return true;
 }
 
-bool Engine::dtw_weights(const std::vector<int> & req, std::vector<std::vector<float> *> & out) {
+bool Engine::dtw_weights(const std::vector<int> & req, const std::vector<int> & path, std::vector<std::vector<float> *> & out,
+                         std::vector<std::vector<int32_t> *> & tok, std::vector<std::vector<int32_t> *> & time) {
     const HParams & hp = m->hp;
     const int n_req = (int) req.size() / 4, d = hp.n_text_state, Lt = hp.n_text_layer;
     WB_CUDA_OK(cudaSetDevice(m->device));
@@ -722,6 +723,14 @@ bool Engine::dtw_weights(const std::vector<int> & req, std::vector<std::vector<f
     WB_CUDA_OK(cudaEventRecord(ev[5], st));
     if (!dtw_qk_launch(a, st)) return false;
     WB_CUDA_OK(cudaEventRecord(ev[6], st));
+    std::vector<int> preq((size_t) DTW_REQ_INTS * n_req);
+    for (int r = 0; r < n_req; ++r) {
+        int * p = preq.data() + (size_t) DTW_REQ_INTS * r;
+        p[0] = req[4 * r + 2]; p[1] = req[4 * r + 3]; p[2] = dtw_n_heads; p[3] = path[2 * r]; p[4] = path[2 * r + 1];
+    }
+    if (!dtw_paths.enqueue(dtw_out.p, preq, std::vector<int64_t>(off.begin(), off.end() - 1), st)) return false;
+    WB_CUDA_OK(cudaEventRecord(ev[7], st));
+    if (!dtw_paths.fetch(st)) return false;
     for (int r = 0; r < n_req; ++r) {
         std::vector<float> & o = *out[(size_t) r];
         o.resize((size_t) (off[(size_t) r + 1] - off[(size_t) r]));
@@ -729,7 +738,9 @@ bool Engine::dtw_weights(const std::vector<int> & req, std::vector<std::vector<f
     }
     WB_CUDA_OK(cudaStreamSynchronize(st));
     count_d2h((uint64_t) off.back() * sizeof(float));
+    for (int r = 0; r < n_req; ++r) dtw_paths.get(r, *tok[(size_t) r], *time[(size_t) r]);
     { float ms = 0.0f; cudaEventElapsedTime(&ms, ev[5], ev[6]); counter_add(8, ms); counter_add(9, n_req); }
+    { float ms = 0.0f; cudaEventElapsedTime(&ms, ev[6], ev[7]); counter_add(11, ms); }
     return true;
 }
 } // namespace wb

@@ -14,6 +14,7 @@
 #include "wb_gemm.cuh"
 #include "wb_kernels.cuh"
 #include "wb_decode_mk.cuh"
+#include "wb_dtw_kernel.cuh"
 
 namespace wb {
 
@@ -80,8 +81,11 @@ struct Engine {
     bool dtw_set_heads(const std::vector<std::pair<int, int>> & heads);   // (text layer, head) in the context's order; once, before any pass
     bool dtw_reserve(int n_rows);
     // alignment weights of several DTW passes in one launch: req = 4 ints per request (first capture index, slot, tokens, audio positions);
-    // out[r] receives [heads][audio positions][tokens] of request r
-    bool dtw_weights(const std::vector<int> & req, std::vector<std::vector<float> *> & out);
+    // out[r] receives [heads][audio positions][tokens] of request r.  Then the warping paths of all of them on the device (DtwPaths):
+    // path = 2 ints per request (audio positions of the window M, sot_len); tok[r] / time[r] receive request r's path (dtw_path's output)
+    bool dtw_weights(const std::vector<int> & req, const std::vector<int> & path, std::vector<std::vector<float> *> & out,
+                     std::vector<std::vector<int32_t> *> & tok, std::vector<std::vector<int32_t> *> & time);
+    DtwPaths dtw_paths;
     bool use_mk = false;
     int  max_rows = 8;               // rows per decode pass: 64 with the persistent kernel, 8 with the chain
     int  n_sm = 0, mk_prefetch = 61;     // bit0: next-phase weights -> L2; bit2: K / V streams with L2 evict-first priority; bit4: logits one warp per weight tile
@@ -112,7 +116,7 @@ struct Engine {
     void drop_graphs();
 
     // device-event timers of the last encode: [1]=conv (incl. window staging) [2]=encoder [3]=cross  ([0] unused: mel is FrontEnd)
-    cudaEvent_t ev[7] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };   // [5],[6]: decode pass
+    cudaEvent_t ev[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };   // [5],[6]: decode pass / k_dtw_qk; [6],[7]: DTW paths
     float last_ms[4] = { 0, 0, 0, 0 };
 
     ~Engine();

@@ -456,7 +456,8 @@ template <typename F> void run_parallel(int n_threads, F && fn) {
 
 // One extra decoder pass over [sot, (lang), no_timestamps, text tokens of the window's segments, eot].  It is an ordinary decode request of the
 // pool that also captures the cross-attention queries of the alignment heads; the batch it joins computes the softmax weights of every
-// DTW request on the device in one launch (Group::run), then the host DTW (wb_dtw.cpp) runs here, on the state's own thread.
+// DTW request on the device in one launch, and then the warping path of each (normalisation, median filter, mean over heads, DTW and
+// backtrace: DtwPaths, Group::run); only the assignment of the path to the tokens (dtw_assign) runs here, on the state's own thread.
 bool dtw_window(whisper_context & ctx, whisper_state & st, const whisper_full_params & params, int i_segment, int n_segments, int seek, int n_frames) {
     const Vocab & vocab = ctx.vocab;
     const int n_audio_ctx = st.exp_n_audio_ctx > 0 ? st.exp_n_audio_ctx : ctx.model.hp.n_audio_ctx;
@@ -483,13 +484,13 @@ bool dtw_window(whisper_context & ctx, whisper_state & st, const whisper_full_pa
         sreq.mask_bits = &mask_bits; sreq.rowinfo = rowinfo.data();
         make_samp_cfg(ctx, params, sreq.cfg);
     }
-    if (!decode_batch(ctx, st, tokens.data(), pos.data(), seq.data(), want.data(), n, dev ? &sreq : nullptr, n_audio_ctx)) return false;
+    st.dtw_tok.clear(); st.dtw_time.clear();
+    if (!decode_batch(ctx, st, tokens.data(), pos.data(), seq.data(), want.data(), n, dev ? &sreq : nullptr, n_audio_ctx, sot_len, n_frames)) return false;
     if (st.dtw_qk_last.size() != (size_t) n * n_audio_ctx * ctx.dtw_heads.size()) { set_error("dtw: the pass returned no alignment weights"); return false; }
+    st.dtw_last_window[0] = n_frames; st.dtw_last_window[1] = sot_len; st.dtw_last_window[2] = seek; st.dtw_last_window[3]++;
     const int64_t t0 = time_us();
-    std::vector<int32_t> ti, tj;
-    dtw_path(st.dtw_qk_last.data(), n, n_audio_ctx, (int) ctx.dtw_heads.size(), n_frames / 2, sot_len, 7, ti, tj);
-    dtw_assign(ti, tj, seek, vocab.token_eot, st.result_all, i_segment, n_segments);
-    counter_add(10, 1e-3 * (double) (time_us() - t0));           // host DTW ms (wb200_counters)
+    dtw_assign(st.dtw_tok, st.dtw_time, seek, vocab.token_eot, st.result_all, i_segment, n_segments);
+    counter_add(10, 1e-3 * (double) (time_us() - t0));           // host DTW ms (wb200_counters): the assignment of the device's path
     return true;
 }
 } // namespace

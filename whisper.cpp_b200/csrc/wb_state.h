@@ -115,6 +115,8 @@ struct whisper_state {
     // decode leaves all-zero logits, so the transcript is whatever the caller's logits_filter_callback scripts.  It computes nothing and
     // cannot be created through any whisper.h entry point.
     std::vector<float> dtw_qk_last;            // alignment-head weights of the last DTW pass [heads][n_audio_ctx][tokens] (wb200_dbg_last_dtw_qks)
+    std::vector<int32_t> dtw_tok, dtw_time;    // its warping path, computed on the device from those weights (DtwPaths)
+    int dtw_last_window[4] = {0, 0, 0, 0};     // its mel frames, sot_len, seek; DTW passes of the state so far (wb200_dbg_last_dtw_window)
     int dtw_last_shape[3] = {0, 0, 0};
     bool scripted = false;
     std::vector<int> dbg_tok, dbg_pos, dbg_seq; std::vector<int8_t> dbg_want;      // scripted states only: the last decode request (wb200_dbg_last_batch)
@@ -185,6 +187,7 @@ struct Group {
         const int * tokens = nullptr, * pos = nullptr, * seq = nullptr; const int8_t * want = nullptr; int n = 0;   // decode
         const SampReq * samp = nullptr;
         int dtw_n_ctx = 0;                       // > 0: a DTW pass; capture its alignment-head queries and compute its weights over this many audio positions
+        int dtw_sot_len = 0, dtw_n_frames = 0;   // DTW pass: tokens before the no-timestamps token, mel frames of the window (its path)
         const int * x_cells = nullptr, * x_idx = nullptr, * x_nkv = nullptr; int x_ld = 0;   // explicit self-KV cells / attended lists (relative to the state's range) instead of the KvCells bookkeeping: the ggml-backend plugin passes what the host's KQ_mask says
         bool taken = false;                      // (under mu) some thread took the batch that contains this request
         std::atomic<int> done{0};                // futex word: the member sleeps on its OWN request (no shared mutex to re-acquire on wake-up)
@@ -218,6 +221,6 @@ int64_t time_us();
 bool & tls_pcm_is_device();   // set by the batch driver: the next whisper_pcm_to_mel* `samples` pointer is a device pointer
 // decode one batch through the engine with the reference's KV bookkeeping (whisper_decode_internal, whisper.cpp:2856-2986)
 bool decode_batch(whisper_context & ctx, whisper_state & st, const int * tokens, const int * pos, const int * seq,
-                  const int8_t * want, int n_tokens, const SampReq * samp = nullptr, int dtw_n_ctx = 0);
+                  const int8_t * want, int n_tokens, const SampReq * samp = nullptr, int dtw_n_ctx = 0, int dtw_sot_len = 0, int dtw_n_frames = 0);
 bool encode_window(whisper_context & ctx, whisper_state & st, int mel_offset);
 }
