@@ -443,7 +443,7 @@ WB_EXPORT void wb200_profile_enable(int on);
 WB_EXPORT void wb200_profile_collect(double * ms4, uint64_t * launches4, double * bytes4, double * flops4);
 /* coarse engine counters since load: [0] decode passes [1] decode rows [2] decode GPU ms [3] decode host ms [4] encode calls
  * [5] encode windows [6] encode GPU ms [7] CUDA-graph replays [8] alignment-weight (k_dtw_qk) GPU ms [9] DTW passes
- * [10] host DTW ms */
+ * [10] host DTW ms [11] device DTW path GPU ms [12] run-ahead decode rows launched [13] run-ahead rows whose results were taken */
 WB_EXPORT void wb200_counters(double * out, int n);
 /* bytes this library has copied host->device / device->host since load */
 WB_EXPORT void wb200_traffic(uint64_t * h2d, uint64_t * d2h);

@@ -6,7 +6,9 @@ per chunk, ONE whisper_full_parallel(ctx, params, pcm, n, 64) call per timed run
 Arms are given as name[:KEY=VALUE,...]; a key is an environment switch read when the context is created, or LIB=<path> for another build
 of the same ABI.  Repeats alternate the arms (a, b, c, a, b, c, ...) so that the run-to-run spread is visible next to the differences.
 Per run: xRT, decode passes, rows per pass, decode GPU ms per pass (wb200_counters [0]-[2]), encode GPU ms per window ([5], [6]), the card
-and its power limit, and whether the token ids and probabilities of all chunks equal those of the first arm.
+and its power limit, and whether the token ids and probabilities of all chunks equal those of the first arm; the wall time no GPU work
+covers (wall - passes x decode GPU ms - windows x encode GPU ms: host turnaround between passes) and the run-ahead rows launched and
+taken (wb200_counters [12], [13]; a build without run-ahead reports zeros).
 --trace ARM: one more, untimed run of that arm with WB200_MK_TRACE set; prints the per-phase split of a layer (us, CTA 0).
 
   python scripts/bench_decode.py --repeats 2 --arms parts1:WB200_MK_PARTS=1 parts2:WB200_MK_PARTS=2 parts4:WB200_MK_PARTS=4 \\
@@ -60,8 +62,8 @@ def card():
 
 
 def counters(L):
-    a = (C.c_double * 8)(); L.wb200_counters(a, 8)
-    return [a[i] for i in range(8)]
+    a = (C.c_double * 14)(); L.wb200_counters(a, 14)
+    return [a[i] for i in range(14)]
 
 
 def outputs(L, ctx):
@@ -103,9 +105,11 @@ def run(pkg, model, env, pcm, n_chunks, trace=None):
     ids, ps = outputs(L, eng.ctx)
     eng.close()                                                  # the trace is written when the engine goes away
     passes = c1[0] - c0[0]
+    gpu_ms = (c1[2] - c0[2]) + (c1[6] - c0[6])                       # decode passes + encoder windows, from their own events
     return {"xRT": len(pcm) / 16000.0 / dt, "wall_s": dt, "decode_passes": passes, "rows_per_pass": (c1[1] - c0[1]) / max(1.0, passes),
             "decode_gpu_ms_per_pass": (c1[2] - c0[2]) / max(1.0, passes), "encode_gpu_ms_per_window": (c1[6] - c0[6]) / max(1.0, c1[5] - c0[5]),
-            "decoded_tokens": int(len(ids))}, ids, ps
+            "uncovered_ms": 1e3 * dt - gpu_ms, "uncovered_frac": 1.0 - gpu_ms / (1e3 * dt),
+            "run_ahead_rows": c1[12] - c0[12], "run_ahead_taken": c1[13] - c0[13], "decoded_tokens": int(len(ids))}, ids, ps
 
 
 def main():
@@ -144,6 +148,8 @@ def main():
         rs = summary[name]
         ms = [r["decode_gpu_ms_per_pass"] for r in rs]; x = [r["xRT"] for r in rs]
         print(json.dumps({"summary": name, "gpu": gpu, "decode_gpu_ms_per_pass": ms, "decode_gpu_ms_per_pass_mean": float(np.mean(ms)),
+                          "uncovered_ms": [r["uncovered_ms"] for r in rs], "uncovered_frac": [r["uncovered_frac"] for r in rs],
+                          "run_ahead_rows": [r["run_ahead_rows"] for r in rs], "run_ahead_taken": [r["run_ahead_taken"] for r in rs],
                           "encode_gpu_ms_per_window": [r["encode_gpu_ms_per_window"] for r in rs],
                           "xRT": x, "xRT_mean": float(np.mean(x)), "rows_per_pass": rs[-1]["rows_per_pass"], "decode_passes": rs[-1]["decode_passes"],
                           "same_as_first_arm": all(r["same_tokens_as_first_arm"] and r["same_probabilities_as_first_arm"] for r in rs)}), flush=True)

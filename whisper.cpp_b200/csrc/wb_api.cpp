@@ -97,8 +97,7 @@ namespace {
 struct PreparedDecode {
     std::vector<DecToken> rows; std::vector<int> cells, nkv, idx; int ld = 0;
 };
-bool prepare_decode(whisper_state & st, const int * tokens, const int * pos, const int * seq, const int8_t * want, int n_tokens, PreparedDecode & P) {
-    KvCells & kv = st.kv;
+bool prepare_rows(KvCells & kv, const whisper_state & st, const int * tokens, const int * pos, const int * seq, const int8_t * want, int n_tokens, PreparedDecode & P) {
     if (!kv.find_slot(pos, seq, (uint32_t) n_tokens)) { set_error("decode: no KV slot for %d tokens", n_tokens); return false; }
     kv.n = (uint32_t) std::min<int>((int) kv.size, std::max(1, kv.cell_max()));      // padding 1 on this path (whisper.cpp:2884-2885)
     const int n_kv = (int) kv.n;
@@ -115,6 +114,9 @@ bool prepare_decode(whisper_state & st, const int * tokens, const int * pos, con
         P.nkv[j] = c;
     }
     return true;
+}
+bool prepare_decode(whisper_state & st, const int * tokens, const int * pos, const int * seq, const int8_t * want, int n_tokens, PreparedDecode & P) {
+    return prepare_rows(st.kv, st, tokens, pos, seq, want, n_tokens, P);
 }
 // test hook (engine-less states): per row a hash of the positions it attends to, i.e. of the index list the kernels would get
 void scripted_attended(whisper_state & st, const PreparedDecode & P, int n_tokens) {
@@ -206,6 +208,7 @@ static int pool_cells_for(const Model & m, int n_decoders) {                    
 // states blocked in submit() keep their slot contents (Engine::resize copies them).
 bool Group::grow_locked(std::unique_lock<std::mutex> & lk, int new_cap, int new_cps) {
     cv.wait(lk, [&] { return !running; });
+    spec_drop();                                                                     // the relayout moves cells and cell_off
     if (!scripted) {
         if (cap == 0) {
             if (!eng.init(model, 1)) return false;                                   // one slot, GGML_PAD(n_text_ctx, 256) cells
@@ -256,6 +259,8 @@ void Group::detach(whisper_state * st) {
 
 bool Group::ensure_cells(whisper_state * st, int cells) {
     std::unique_lock<std::mutex> lk(mu);
+    cv.wait(lk, [&] { return !running; });
+    spec_drop();                                                                     // kv.reset below rewrites the state's cell table
     if (cells > cps) {
         // another state may hold cells beyond `cells` only if cps already covered them, so growing never truncates anybody
         if (!grow_locked(lk, cap, cells)) return false;
@@ -351,6 +356,11 @@ GroupCall::~GroupCall() {
     if (suspended) suspended->group->resume(suspended);
 }
 
+void Group::spec_drop() {
+    if (!scripted) for (int s = 0; s < Engine::PASS_SLOTS; ++s) eng.pass_wait(s);
+    spec_pass = -1; spec_rows.clear();
+}
+
 void Group::run(std::vector<Req *> & batch) {
     for (Req * q : batch) q->st->cell_off = q->st->slot * cps;      // the pool may have been re-laid out since the request was queued
     // encode requests first (they only touch the encoder workspaces and the members' cross-KV slots)
@@ -426,22 +436,45 @@ void Group::run(std::vector<Req *> & batch) {
         } else {
         if (ok && all_samp) ok = eng.set_samp_mask(cfg0->samp->mask_key, *cfg0->samp->mask_bits);
         if (ok && n_cap > 0) ok = eng.dtw_reserve(n_cap);
+        // run-ahead: greedy rows of one decoder, sampled on the device, on the persistent kernel; never while per-launch profiling or
+        // tracing is on (those runs attribute every launch to its pass), never with DTW (its passes capture queries and sample nothing)
+        int stride = 1;                                                // entries per row of the sampler output: the widest request decides
+        auto own_stride = [](const Req * q) { return (q->samp && q->samp->draws) ? q->samp->stride : 1; };
+        if (all_samp) for (Req * q : dec) stride = std::max(stride, own_stride(q));
+        const bool ahead = ok && run_ahead && all_samp && stride == 1 && n_cap == 0 && dtw_heads.empty() && eng.use_mk && !prof_enabled() && !eng.mk_trace.p;
+        // requests the queued run-ahead pass already computed: acc[i] = its row, -1: run in an ordinary pass
+        std::vector<int> acc(dec.size(), -1);
+        int n_acc = 0;
+        if (ahead && spec_pass >= 0 && spec_mask_key == cfg0->samp->mask_key && same_cfg(spec_cfg, cfg0->samp->cfg)) {
+            for (size_t i = 0; i < dec.size(); ++i) {
+                const Req * q = dec[i]; const PreparedDecode & P = preps[i];
+                if (q->n != 1 || q->x_cells || q->dtw_n_ctx || !q->want[0] || q->samp->draws) continue;
+                for (size_t k = 0; k < spec_rows.size(); ++k) {
+                    const SpecRow & r = spec_rows[k];
+                    if (r.st != q->st) continue;
+                    if (r.token == q->tokens[0] && r.pos == q->pos[0] && r.seq == q->seq[0] && r.slot == q->st->slot && r.cell == P.cells[0] &&
+                        r.n_ctx == eng.slot_n_ctx(r.slot) && (r.rowinfo[0] & 0xff) == (q->samp->rowinfo[0] & 0xff) && r.rowinfo[1] == q->samp->rowinfo[1] &&
+                        (int) r.idx.size() == P.nkv[0] && std::equal(r.idx.begin(), r.idx.end(), P.idx.begin())) { acc[i] = (int) k; ++n_acc; }
+                    break;
+                }
+            }
+        }
         if (ok) {
-            int stride = 1;                                            // entries per row of the sampler output: the widest request decides
-            auto own_stride = [](const Req * q) { return (q->samp && q->samp->draws) ? q->samp->stride : 1; };
-            if (all_samp) for (Req * q : dec) stride = std::max(stride, own_stride(q));
             std::vector<int> cap0(dec.size(), -1);
             for (size_t i = 0, c = 0; i < dec.size(); ++i) if (dec[i]->dtw_n_ctx > 0) { cap0[i] = dtw_req[4 * c]; ++c; }
             for (Req * q : dec) { if (all_samp) { q->st->samp_stride = own_stride(q); q->st->samp_out.assign((size_t) q->n * q->st->samp_stride, SampOut()); } else { q->st->samp_out.clear(); q->st->logits.resize((size_t) q->n * n_vocab); } }
             // one decode call per encoded context length (a pass attends to one number of cross keys), requests in slot order within each
             std::vector<std::vector<size_t>> groups; std::vector<int> group_ctx;
             for (size_t i = 0; i < dec.size(); ++i) {
+                if (acc[i] >= 0) continue;
                 const int T = eng.slot_n_ctx(dec[i]->st->slot);
                 size_t g = 0;
                 while (g < groups.size() && group_ctx[g] != T) ++g;
                 if (g == groups.size()) { groups.emplace_back(); group_ctx.push_back(T); }
                 groups[g].push_back(i);
             }
+            // with run-ahead, a batch whose ordinary rows fit one pass only enqueues it here: the next run-ahead pass goes in behind it
+            int o_pass = -1; std::vector<std::pair<Req *, int>> o_origin;
             for (const std::vector<size_t> & grp : groups) {
                 if (!ok) break;
                 int gtotal = 0; for (size_t i : grp) gtotal += dec[i]->n;
@@ -471,7 +504,11 @@ void Group::run(std::vector<Req *> & batch) {
                         origin.emplace_back(q, k);
                     }
                 }
-                if (all_samp) {
+                if (ahead && groups.size() == 1 && gtotal <= eng.max_rows) {
+                    ok = eng.pass_enqueue(rows.data(), gtotal, cells.data(), idx.data(), ld, nkv.data(), &cfg0->samp->cfg, rowinfo.data(), nullptr, 1,
+                                          nullptr, nullptr, &o_pass);
+                    o_origin.swap(origin);
+                } else if (all_samp) {
                     ok = eng.decode(rows.data(), gtotal, cells.data(), idx.data(), ld, nkv.data(), nullptr, &cfg0->samp->cfg, rowinfo.data(), souts.data(),
                                     stride > 1 ? draws.data() : nullptr, stride, n_cap > 0 ? capidx.data() : nullptr);
                     for (int r = 0; r < gtotal; ++r) {
@@ -483,6 +520,71 @@ void Group::run(std::vector<Req *> & batch) {
                                     n_cap > 0 ? capidx.data() : nullptr);
                 }
             }
+            // the next run-ahead pass: the single-token step after the last row of every request whose member may continue, its token
+            // taken on the device from this batch's sampler output (the accepted run-ahead rows, or the ordinary pass enqueued above)
+            // A mispredicted row costs a whole ordinary pass behind the run-ahead pass (two passes for the step instead of one), a
+            // taken pass saves one host turnaround.  Where predictions fail often (timestamps sampled every few tokens) the pool runs
+            // lock-step and tries again every 256th batch: spec_miss is the running share of run-ahead batches with a mispredicted row.
+            if (spec_pass >= 0) {
+                bool miss = false;
+                for (size_t i = 0; i < dec.size() && !miss; ++i)
+                    if (acc[i] < 0 && dec[i]->n == 1)
+                        for (const SpecRow & r : spec_rows) miss |= r.st == dec[i]->st;
+                spec_miss += ((miss ? 1.0f : 0.0f) - spec_miss) / 8.0f;
+            }
+            const bool try_ahead = spec_miss < 0.25f || ++spec_idle >= 256;
+            int next_pass = -1; std::vector<SpecRow> next;
+            if (ok && ahead && try_ahead) {
+                auto predict = [&](Req * q, int src_pass, int src_row) {
+                    const int k = q->n - 1;
+                    if (!q->samp->next_step || q->x_cells || !q->want[k] || q->seq[k] != 0) return;
+                    KvCells kv = q->st->kv;                               // what find_slot and the KQ-mask rule will give the real request
+                    const int pos = q->pos[k] + 1, seq = 0, tok = 0; const int8_t want = 1;
+                    PreparedDecode P;
+                    if (pos >= q->ctx->model.hp.n_text_ctx || !prepare_rows(kv, *q->st, &tok, &pos, &seq, &want, 1, P)) return;
+                    SpecRow r{ q->st, -1, pos, seq, q->st->slot, P.cells[0], eng.slot_n_ctx(q->st->slot), { q->samp->next_rowinfo[0], q->samp->next_rowinfo[1] },
+                               std::vector<int>(P.idx.begin(), P.idx.begin() + P.nkv[0]), src_pass, src_row };
+                    next.push_back(std::move(r));
+                };
+                for (size_t i = 0; i < dec.size(); ++i) if (acc[i] >= 0) predict(dec[i], spec_pass, acc[i]);
+                for (size_t r = 0; r < o_origin.size(); ++r) if (o_origin[r].second == o_origin[r].first->n - 1) predict(o_origin[r].first, o_pass, (int) r);
+                bool one_ctx = true;
+                for (const SpecRow & r : next) one_ctx &= r.n_ctx == next[0].n_ctx;
+                if (!next.empty() && one_ctx && (int) next.size() <= eng.max_rows) {
+                    std::sort(next.begin(), next.end(), [](const SpecRow & a, const SpecRow & b) { return a.slot < b.slot; });   // row order of a pass
+                    const int nn = (int) next.size();
+                    int nld = 1; for (const SpecRow & r : next) nld = std::max(nld, (int) r.idx.size());
+                    std::vector<DecToken> rows; std::vector<int> cells, nkv, idx((size_t) nn * nld, 0), rowinfo, src;
+                    for (int j = 0; j < nn; ++j) {
+                        const SpecRow & r = next[j];
+                        rows.push_back({ 0, r.pos, r.seq, r.slot, true }); cells.push_back(r.cell); nkv.push_back((int) r.idx.size());
+                        std::copy(r.idx.begin(), r.idx.end(), idx.begin() + (size_t) j * nld);
+                        rowinfo.push_back(r.rowinfo[0] & 0xff); rowinfo.push_back(r.rowinfo[1]);
+                        src.push_back((int) (eng.dsamp_of(r.src_pass) - eng.dsamp.p) + r.src_row);   // stride-1 passes: entry 0 of row src_row
+                    }
+                    ok = eng.pass_enqueue(rows.data(), nn, cells.data(), idx.data(), nld, nkv.data(), &cfg0->samp->cfg, rowinfo.data(), nullptr, 1,
+                                          nullptr, src.data(), &next_pass);
+                    if (ok) counter_add(12, nn);
+                    spec_idle = 0;
+                } else {
+                    next.clear();
+                }
+            }
+            // results: the accepted rows of the previous run-ahead pass, then the ordinary pass; each fills in the tokens it fed forward
+            auto harvest = [&](int pass) {
+                if (pass < 0) return;
+                if (!eng.pass_wait(pass)) { ok = false; return; }
+                for (SpecRow & r : next) if (r.src_pass == pass) r.token = eng.pslot[pass].hsamp[r.src_row].id;
+            };
+            if (spec_pass >= 0) {
+                harvest(spec_pass);
+                if (ok) for (size_t i = 0; i < dec.size(); ++i) if (acc[i] >= 0) dec[i]->st->samp_out[0] = eng.pslot[spec_pass].hsamp[acc[i]];
+                counter_add(13, n_acc);
+            }
+            harvest(o_pass);
+            if (ok) for (size_t r = 0; r < o_origin.size(); ++r) o_origin[r].first->st->samp_out[(size_t) o_origin[r].second] = eng.pslot[o_pass].hsamp[r];
+            spec_pass = -1; spec_rows.clear();
+            if (ok && next_pass >= 0) { spec_pass = next_pass; spec_rows.swap(next); spec_mask_key = cfg0->samp->mask_key; spec_cfg = cfg0->samp->cfg; }
             // alignment weights and warping paths of every DTW request of the batch, one launch per kernel (dtw_assign runs on each state's
             // own thread)
             if (ok && n_cap > 0) {
@@ -492,6 +594,7 @@ void Group::run(std::vector<Req *> & batch) {
                 for (Req * q : dtw_of) { whisper_state & s = *q->st; s.dtw_last_shape[0] = q->n; s.dtw_last_shape[1] = q->dtw_n_ctx; s.dtw_last_shape[2] = eng.dtw_n_heads; }
             }
         }
+        if (!ok) spec_drop();
         }
         const int64_t dt = (time_us() - t0) / (int64_t) dec.size();
         for (Req * q : dec) { q->ok = ok; q->dt_us = dt; }
@@ -650,10 +753,10 @@ WB_EXPORT struct whisper_state * whisper_init_state(struct whisper_context * ctx
         Group * pool = nullptr; const Model * model = &ctx->model;
         {
             std::lock_guard<std::mutex> lk(ctx->replicas_mu);
-            if (!ctx->pool) { ctx->pool.reset(new Group()); ctx->pool->model = &ctx->model; ctx->pool->scripted = ctx->scripted; ctx->pool->dtw_heads = ctx->dtw_heads; }
+            if (!ctx->pool) { ctx->pool.reset(new Group()); ctx->pool->model = &ctx->model; ctx->pool->scripted = ctx->scripted; ctx->pool->dtw_heads = ctx->dtw_heads; ctx->pool->run_ahead = ctx->run_ahead; }
             pool = ctx->pool.get();
             for (auto & r : ctx->replicas) {
-                if (!r->pool) { r->pool.reset(new Group()); r->pool->model = &r->model; }
+                if (!r->pool) { r->pool.reset(new Group()); r->pool->model = &r->model; r->pool->run_ahead = ctx->run_ahead; }
                 if (r->pool->n_registered < pool->n_registered) { pool = r->pool.get(); model = &r->model; }
             }
         }
@@ -1088,6 +1191,14 @@ WB_EXPORT int wb200_pcm_upload(struct whisper_state * st, const float * samples,
 }
 WB_EXPORT void wb200_profile_enable(int on) { wb::prof_enable(on != 0); }
 WB_EXPORT void wb200_profile_collect(double * ms4, uint64_t * launches4, double * bytes4, double * flops4) { wb::prof_collect(ms4, launches4, bytes4, flops4); }
+// test hook: run-ahead decode passes on (default) or off for every pool of the context, so that tests can compare both in one process
+WB_EXPORT int wb200_dbg_run_ahead(struct whisper_context * ctx, int on) {
+    if (!ctx) return -1;
+    ctx->run_ahead = on != 0;
+    if (ctx->pool) ctx->pool->run_ahead = on != 0;
+    for (auto & r : ctx->replicas) if (r->pool) r->pool->run_ahead = on != 0;
+    return 0;
+}
 WB_EXPORT void wb200_counters(double * out, int n) { for (int i = 0; i < n && i < 16; ++i) out[i] = wb::counter_get(i); }
 WB_EXPORT void wb200_traffic(uint64_t * h2d, uint64_t * d2h) { if (h2d) *h2d = wb::h2d_bytes(); if (d2h) *d2h = wb::d2h_bytes(); }
 WB_EXPORT const char * wb200_last_error(void) { return wb::last_error(); }

@@ -34,6 +34,7 @@ void prof_collect(double * ms, uint64_t * launches, double * bytes, double * flo
 // coarse engine counters (wb200_counters): [0] decode passes [1] decode rows [2] decode GPU ms (events around each pass)
 // [3] decode host ms (wall time inside Engine::decode) [4] encode calls [5] encode windows [6] encode GPU ms [7] graph replays
 // [8] k_dtw_qk GPU ms [9] DTW passes [10] host DTW ms (dtw_assign) [11] device DTW path GPU ms (k_dtw_norm, k_dtw_cost, k_dtw_sweep)
+// [12] run-ahead decode rows launched (Group::run) [13] run-ahead rows accepted, i.e. whose results a member's real request took
 void   counter_add(int idx, double v);
 double counter_get(int idx);
 

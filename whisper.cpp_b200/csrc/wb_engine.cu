@@ -27,12 +27,17 @@ void Engine::drop_graphs() {
 
 Engine::~Engine() {
     if (m) cudaSetDevice(m->device);
+    if (st) cudaStreamSynchronize(st);                            // a run-ahead pass may still be queued
     mk_trace_dump();
     drop_graphs();
     delete plan;
-    if (hints) cudaFreeHost(hints);
+    for (PassSlot & s : pslot) {
+        if (s.hints) cudaFreeHost(s.hints);
+        if (s.hsamp) cudaFreeHost(s.hsamp);
+        if (s.ev0) cudaEventDestroy(s.ev0);
+        if (s.ev1) cudaEventDestroy(s.ev1);
+    }
     if (hlogits) cudaFreeHost(hlogits);
-    if (hsamp) cudaFreeHost(hsamp);
     if (hdraws) cudaFreeHost(hdraws);
     for (auto & e : ev) if (e) cudaEventDestroy(e);
     if (st) cudaStreamDestroy(st);
@@ -43,6 +48,7 @@ bool Engine::init(const Model * model, int cap_windows) {
     WB_CUDA_OK(cudaSetDevice(m->device));
     WB_CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     for (auto & e : ev) WB_CUDA_OK(cudaEventCreate(&e));
+    for (PassSlot & s : pslot) { WB_CUDA_OK(cudaEventCreate(&s.ev0)); WB_CUDA_OK(cudaEventCreate(&s.ev1)); }
     const HParams & hp = m->hp;
     const int d = hp.n_audio_state, H = hp.n_audio_head, T = hp.n_audio_ctx, Tp = pad256(T), M = hp.n_mels, Lt = hp.n_text_layer, V = hp.n_vocab;
     const size_t B = cap_win;
@@ -85,9 +91,9 @@ bool Engine::init(const Model * model, int cap_windows) {
     if (!act_scratch.alloc(8 * act_tok_stride(m->wtype == WT_F32 ? WT_F16 : m->wtype, 4 * d) + 256)) return false;
     if (!set_cells(pad256(hp.n_text_ctx))) return false;
     WB_CUDA_OK(cudaMallocHost(&hlogits, (size_t) max_rows * V * sizeof(float)));
-    WB_CUDA_OK(cudaMallocHost(&hsamp, (size_t) max_rows * SAMP_MAX_DRAWS * sizeof(SampOut)));
+    for (PassSlot & s : pslot) WB_CUDA_OK(cudaMallocHost(&s.hsamp, (size_t) max_rows * SAMP_MAX_DRAWS * sizeof(SampOut)));
     WB_CUDA_OK(cudaMallocHost(&hdraws, (size_t) max_rows * SAMP_MAX_DRAWS * sizeof(double)));
-    if (!dsamp.alloc((size_t) max_rows * SAMP_MAX_DRAWS) || !ddraws.alloc((size_t) max_rows * SAMP_MAX_DRAWS) || !samp_mask.alloc((size_t) (V + 31) / 32, true)) return false;
+    if (!dsamp.alloc((size_t) PASS_SLOTS * max_rows * SAMP_MAX_DRAWS) || !ddraws.alloc((size_t) max_rows * SAMP_MAX_DRAWS) || !samp_mask.alloc((size_t) (V + 31) / 32, true)) return false;
     return true;
 }
 
@@ -145,6 +151,7 @@ bool Engine::resize(int new_cap, int new_cps) {
 bool Engine::set_cells(int n) {
     const HParams & hp = m->hp;
     WB_CUDA_OK(cudaSetDevice(m->device));
+    WB_CUDA_OK(cudaStreamSynchronize(st));                        // queued passes read the buffers and row tables replaced here
     drop_graphs();
     n_cells = n; cps = n / std::max(1, cap_win);
     const size_t e = (size_t) hp.n_text_layer * n * hp.n_text_state;
@@ -152,9 +159,11 @@ bool Engine::set_cells(int n) {
     ld_idx = pad256(hp.n_text_ctx);          // a query attends to at most n_text_ctx positions
     const size_t nints = (size_t) max_rows * (8 + ld_idx);
     if (!dints.alloc(nints)) return false;
-    if (hints) cudaFreeHost(hints);
-    hints = nullptr;
-    WB_CUDA_OK(cudaMallocHost(&hints, nints * sizeof(int)));
+    for (PassSlot & s : pslot) {
+        if (s.hints) cudaFreeHost(s.hints);
+        s.hints = nullptr;
+        WB_CUDA_OK(cudaMallocHost(&s.hints, nints * sizeof(int)));
+    }
     if (use_mk && !mk_build_table()) return false;
     return true;
 }
@@ -469,7 +478,7 @@ bool Engine::set_samp_mask(uint64_t key, const std::vector<uint32_t> & bits) {
     return true;
 }
 
-bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp) {
+bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp, bool tok_indirect) {
     const HParams & hp = m->hp;
     const int d = hp.n_text_state, H = hp.n_text_head, Lt = hp.n_text_layer, V = hp.n_vocab;
     const int Tp = Tp_max;                                         // kv_cross layout stride
@@ -481,6 +490,7 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio
     const int * d_cap = dints.p + 7 * R, * d_idx = dints.p + 8 * R;
 
     auto chain_gemv = [&](const GemvArgs & a) { if (gemv_v2) gemv2(a, act_scratch.p, st); else gemv(a, st); };
+    if (tok_indirect) tok_resolve(dints.p, dsamp.p, n, st);
     dec_embed(m->d_te, m->d_pe, d_tok, d_pos, n, d, dx.p, st);
     if (use_mk) {
         MkArgs a;
@@ -558,8 +568,8 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio
         if (samp) {
             SampCfg c = *samp; c.mask = samp_mask.p;
             if (draw_stride > 1) WB_CUDA_OK(cudaMemcpyAsync(ddraws.p, hdraws, (size_t) n * draw_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-            greedy_sample(dlogits.p, V, n, d_row, c, dsamp.p, st, draw_stride > 1 ? ddraws.p : nullptr, draw_stride);
-            WB_CUDA_OK(cudaMemcpyAsync(hsamp, dsamp.p, (size_t) n * draw_stride * sizeof(SampOut), cudaMemcpyDeviceToHost, st));
+            greedy_sample(dlogits.p, V, n, d_row, c, dsamp_of(cur_slot), st, draw_stride > 1 ? ddraws.p : nullptr, draw_stride);
+            WB_CUDA_OK(cudaMemcpyAsync(hsamp, dsamp_of(cur_slot), (size_t) n * draw_stride * sizeof(SampOut), cudaMemcpyDeviceToHost, st));
         } else {
             WB_CUDA_OK(cudaMemcpyAsync(hlogits, dlogits.p, (size_t) n * V * 4, cudaMemcpyDeviceToHost, st));
         }
@@ -567,85 +577,114 @@ bool Engine::decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio
     return true;
 }
 
+bool Engine::pass_enqueue(const DecToken * rows, int n, const int * cells, const int * kv_idx, int ld, const int * n_kv, const SampCfg * samp,
+                          const int * rowinfo, const double * draws, int stride, const int * cap_idx, const int * tok_src, int * slot_out) {
+    const HParams & hp = m->hp;
+    WB_CUDA_OK(cudaSetDevice(m->device));
+    const int V = hp.n_vocab, R = max_rows;
+    if (n < 1 || n > R) { set_error("decode: %d rows in one pass (1..%d)", n, R); return false; }
+    int slot = 0;
+    while (slot < PASS_SLOTS && pslot[slot].busy) ++slot;
+    if (slot == PASS_SLOTS) { set_error("decode: every pass slot is in flight"); return false; }
+    PassSlot & ps = pslot[slot];
+    cur_slot = slot; hints = ps.hints; hsamp = ps.hsamp;
+    int * h_tok = hints, * h_pos = hints + R, * h_cell = hints + 2 * R, * h_slot = hints + 3 * R, * h_nkv = hints + 4 * R, * h_row = hints + 5 * R;
+    int * h_cap = hints + 7 * R, * h_idx = hints + 8 * R;
+    bool any_logits = false, indirect = false;
+    pass_capture = false;
+    for (int j = 0; j < n; ++j) {
+        const DecToken & t = rows[j];
+        const int src = tok_src ? tok_src[j] : -1;
+        if (src >= PASS_SLOTS * R * SAMP_MAX_DRAWS || (src < 0 && (t.token < 0 || t.token >= V)) || t.pos < 0 || t.pos >= hp.n_text_ctx || t.slot < 0 || t.slot >= cap_win) {
+            set_error("decode: bad token/pos/slot (%d, %d, %d)", src >= 0 ? src : t.token, t.pos, t.slot); return false;
+        }
+        if (n_kv[j] > ld_idx || n_kv[j] > ld) { set_error("decode: %d attended cells exceed the index row (%d)", n_kv[j], ld_idx); return false; }
+        h_tok[j] = src >= 0 ? -1 - src : t.token; h_pos[j] = t.pos; h_cell[j] = cells[j]; h_slot[j] = t.slot; h_nkv[j] = n_kv[j];
+        h_row[2*j] = (samp && rowinfo) ? rowinfo[2*j] : 0; h_row[2*j + 1] = (samp && rowinfo) ? rowinfo[2*j + 1] : 0;
+        memcpy(h_idx + (size_t) j * ld_idx, kv_idx + (size_t) j * ld, (size_t) n_kv[j] * sizeof(int));
+        h_cap[j] = cap_idx ? cap_idx[j] : -1;
+        if (h_cap[j] >= dtw_cap_rows) { set_error("decode: capture index %d exceeds the capture buffer (%d rows)", h_cap[j], dtw_cap_rows); return false; }
+        pass_capture |= h_cap[j] >= 0;
+        any_logits |= t.want_logits;
+        indirect |= src >= 0;
+    }
+    const int n_ctx = slot_n_ctx(rows[0].slot), n_keys = pad256(n_ctx);   // encoder positions of the pass's cross K/V
+    for (int j = 1; j < n; ++j)
+        if (slot_n_ctx(rows[j].slot) != n_ctx) {
+            set_error("decode: one pass over slots encoded at %d and %d positions", n_ctx, slot_n_ctx(rows[j].slot)); return false;
+        }
+    draw_stride = (samp && draws && stride > 1) ? std::min(stride, (int) SAMP_MAX_DRAWS) : 1;
+    if (draw_stride > 1) {
+        for (int j = 0; j < n; ++j) memcpy(hdraws + (size_t) j * draw_stride, draws + (size_t) j * stride, (size_t) draw_stride * sizeof(double));
+        for (int j = 0; j < n; ++j) if (((h_row[2*j] >> 8) & 0x7f) > draw_stride) { set_error("decode: a row asks for more draws than the pass carries"); return false; }
+        count_h2d((size_t) n * draw_stride * sizeof(double));
+    } else {
+        for (int j = 0; j < n; ++j) h_row[2*j] &= 0xff;           // no uniforms supplied: greedy picks only
+    }
+    if (indirect && !(use_mk && samp && any_logits)) { set_error("decode: token indirection needs the persistent kernel and the on-device sampler"); return false; }
+    count_h2d(((size_t) 8 * R + (size_t) n * ld_idx) * sizeof(int));
+    if (any_logits) count_d2h(samp ? (uint64_t) n * draw_stride * sizeof(SampOut) : (uint64_t) n * V * 4);
+
+    // One pass = 8 kernels per text layer.  After the second use of a shape the chain is replayed as a CUDA graph
+    // (all per-step values live in `dints`, so kernel arguments never change between steps).
+    uint64_t key = (uint64_t) (n | (any_logits ? 128 : 0) | (samp ? 256 : 0)) | ((uint64_t) n_keys << 10) | ((uint64_t) draw_stride << 24);
+    if (samp) key |= (uint64_t) ((uint32_t) (samp->token_eot * 31 + samp->token_beg * 17 + samp->token_nosp * 13 + samp->space_id * 7 + samp->max_initial_tid * 3 + samp->no_timestamps * 2 + samp->suppress_blank)) << 32;
+    // a graph holds the pinned buffers of the slot it was captured in: only slot 0 replays them (the chain never has two passes in flight)
+    StepGraph * sg = (use_graphs && !use_mk && !prof_enabled() && !pass_capture && slot == 0) ? &graphs[key] : nullptr;
+    WB_CUDA_OK(cudaEventRecord(ps.ev0, st));
+    if (sg && sg->exec) {
+        WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
+        count_launch(sg->launches);
+        counter_add(7, 1);
+    } else if (sg && sg->seen >= 1) {
+        const uint64_t l0 = launch_count();
+        cudaGraph_t g = nullptr;
+        WB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+        const bool ok = decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp);
+        const cudaError_t ce = cudaStreamEndCapture(st, &g);
+        if (!ok || ce != cudaSuccess) { if (g) cudaGraphDestroy(g); set_error("decode: graph capture failed: %s", cudaGetErrorString(ce)); return false; }
+        sg->launches = launch_count() - l0;
+        const cudaError_t ie = cudaGraphInstantiate(&sg->exec, g, 0);
+        cudaGraphDestroy(g);
+        if (ie != cudaSuccess) { sg->exec = nullptr; set_error("decode: cudaGraphInstantiate: %s", cudaGetErrorString(ie)); return false; }
+        WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
+    } else {
+        if (sg) sg->seen++;
+        if (!decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp, indirect)) return false;
+    }
+    WB_CUDA_OK(cudaEventRecord(ps.ev1, st));
+    ps.busy = true; ps.n = n; ps.draw_stride = draw_stride; ps.any_logits = any_logits;
+    *slot_out = slot;
+    return true;
+}
+
+bool Engine::pass_wait(int slot) {
+    PassSlot & ps = pslot[slot];
+    if (!ps.busy) return true;
+    WB_CUDA_OK(cudaSetDevice(m->device));
+    ps.busy = false;
+    WB_CUDA_OK(cudaEventSynchronize(ps.ev1));
+    { float ms = 0.0f; cudaEventElapsedTime(&ms, ps.ev0, ps.ev1); counter_add(0, 1); counter_add(1, ps.n); counter_add(2, ms); }
+    if (use_mk && mk_trace.p && ps.any_logits) mk_trace_collect(m->hp.n_text_layer, true);
+    return true;
+}
+
 bool Engine::decode(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, float * const * logits_out,
                     const SampCfg * samp, const int * rowinfo, SampOut * samp_out, const double * draws, int stride, const int * cap_idx) {
     NvtxRange nvtx("wb200.decode");
-    const HParams & hp = m->hp;
-    WB_CUDA_OK(cudaSetDevice(m->device));
-    const int V = hp.n_vocab;
-
+    const int V = m->hp.n_vocab;
     const int64_t t_host0 = std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
-    const int R = max_rows;
-    for (int r0 = 0; r0 < n_rows; r0 += R) {
-        const int n = std::min(R, n_rows - r0);
-        int * h_tok = hints, * h_pos = hints + R, * h_cell = hints + 2 * R, * h_slot = hints + 3 * R, * h_nkv = hints + 4 * R, * h_row = hints + 5 * R;
-        int * h_cap = hints + 7 * R, * h_idx = hints + 8 * R;
-        bool any_logits = false;
-        pass_capture = false;
-        for (int j = 0; j < n; ++j) {
-            const DecToken & t = rows[r0 + j];
-            if (t.token < 0 || t.token >= V || t.pos < 0 || t.pos >= hp.n_text_ctx || t.slot < 0 || t.slot >= cap_win) {
-                set_error("decode: bad token/pos/slot (%d, %d, %d)", t.token, t.pos, t.slot); return false;
-            }
-            if (n_kv[r0 + j] > ld_idx || n_kv[r0 + j] > ld) { set_error("decode: %d attended cells exceed the index row (%d)", n_kv[r0 + j], ld_idx); return false; }
-            h_tok[j] = t.token; h_pos[j] = t.pos; h_cell[j] = cells[r0 + j]; h_slot[j] = t.slot; h_nkv[j] = n_kv[r0 + j];
-            h_row[2*j] = (samp && rowinfo) ? rowinfo[2*(r0 + j)] : 0; h_row[2*j + 1] = (samp && rowinfo) ? rowinfo[2*(r0 + j) + 1] : 0;
-            memcpy(h_idx + (size_t) j * ld_idx, kv_idx + (size_t) (r0 + j) * ld, (size_t) n_kv[r0 + j] * sizeof(int));
-            h_cap[j] = cap_idx ? cap_idx[r0 + j] : -1;
-            if (h_cap[j] >= dtw_cap_rows) { set_error("decode: capture index %d exceeds the capture buffer (%d rows)", h_cap[j], dtw_cap_rows); return false; }
-            pass_capture |= h_cap[j] >= 0;
-            any_logits |= t.want_logits;
-        }
-        const int n_ctx = slot_n_ctx(rows[r0].slot), n_keys = pad256(n_ctx);   // encoder positions of the pass's cross K/V
-        for (int j = 1; j < n; ++j)
-            if (slot_n_ctx(rows[r0 + j].slot) != n_ctx) {
-                set_error("decode: one pass over slots encoded at %d and %d positions", n_ctx, slot_n_ctx(rows[r0 + j].slot)); return false;
-            }
-        draw_stride = (samp && draws && stride > 1) ? std::min(stride, (int) SAMP_MAX_DRAWS) : 1;
-        if (draw_stride > 1) {
-            for (int j = 0; j < n; ++j) memcpy(hdraws + (size_t) j * draw_stride, draws + (size_t) (r0 + j) * stride, (size_t) draw_stride * sizeof(double));
-            for (int j = 0; j < n; ++j) if (((h_row[2*j] >> 8) & 0x7f) > draw_stride) { set_error("decode: a row asks for more draws than the pass carries"); return false; }
-            count_h2d((size_t) n * draw_stride * sizeof(double));
-        } else {
-            for (int j = 0; j < n; ++j) h_row[2*j] &= 0xff;           // no uniforms supplied: greedy picks only
-        }
-        count_h2d(((size_t) 8 * R + (size_t) n * ld_idx) * sizeof(int));
-        if (any_logits) count_d2h(samp ? (uint64_t) n * draw_stride * sizeof(SampOut) : (uint64_t) n * V * 4);
-
-        // One pass = 8 kernels per text layer.  After the second use of a shape the chain is replayed as a CUDA graph
-        // (all per-step values live in `dints`, so kernel arguments never change between steps).
-        uint64_t key = (uint64_t) (n | (any_logits ? 128 : 0) | (samp ? 256 : 0)) | ((uint64_t) n_keys << 10) | ((uint64_t) draw_stride << 24);
-        if (samp) key |= (uint64_t) ((uint32_t) (samp->token_eot * 31 + samp->token_beg * 17 + samp->token_nosp * 13 + samp->space_id * 7 + samp->max_initial_tid * 3 + samp->no_timestamps * 2 + samp->suppress_blank)) << 32;
-        StepGraph * sg = (use_graphs && !use_mk && !prof_enabled() && !pass_capture) ? &graphs[key] : nullptr;
-        WB_CUDA_OK(cudaEventRecord(ev[5], st));
-        if (sg && sg->exec) {
-            WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
-            count_launch(sg->launches);
-            counter_add(7, 1);
-        } else if (sg && sg->seen >= 1) {
-            const uint64_t l0 = launch_count();
-            cudaGraph_t g = nullptr;
-            WB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const bool ok = decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp);
-            const cudaError_t ce = cudaStreamEndCapture(st, &g);
-            if (!ok || ce != cudaSuccess) { if (g) cudaGraphDestroy(g); set_error("decode: graph capture failed: %s", cudaGetErrorString(ce)); return false; }
-            sg->launches = launch_count() - l0;
-            const cudaError_t ie = cudaGraphInstantiate(&sg->exec, g, 0);
-            cudaGraphDestroy(g);
-            if (ie != cudaSuccess) { sg->exec = nullptr; set_error("decode: cudaGraphInstantiate: %s", cudaGetErrorString(ie)); return false; }
-            WB_CUDA_OK(cudaGraphLaunch(sg->exec, st));
-        } else {
-            if (sg) sg->seen++;
-            if (!decode_pass_enqueue(n, any_logits, n_keys, n_ctx, samp)) return false;
-        }
-        WB_CUDA_OK(cudaEventRecord(ev[6], st));
-        WB_CUDA_OK(cudaStreamSynchronize(st));
-        { float ms = 0.0f; cudaEventElapsedTime(&ms, ev[5], ev[6]); counter_add(0, 1); counter_add(1, n); counter_add(2, ms); }
-        if (use_mk && mk_trace.p && any_logits) mk_trace_collect(hp.n_text_layer, true);
-        if (any_logits && samp && samp_out) {
+    for (int r0 = 0; r0 < n_rows; r0 += max_rows) {
+        const int n = std::min(max_rows, n_rows - r0);
+        int slot = 0;
+        if (!pass_enqueue(rows + r0, n, cells + r0, kv_idx + (size_t) r0 * ld, ld, n_kv + r0, samp, rowinfo ? rowinfo + 2 * r0 : nullptr,
+                          draws ? draws + (size_t) r0 * stride : nullptr, stride, cap_idx ? cap_idx + r0 : nullptr, nullptr, &slot) ||
+            !pass_wait(slot)) return false;
+        const PassSlot & ps = pslot[slot];
+        if (ps.any_logits && samp && samp_out) {
             for (int j = 0; j < n; ++j) if (rows[r0 + j].want_logits)
-                for (int q = 0; q < draw_stride; ++q) samp_out[(size_t) (r0 + j) * stride + q] = hsamp[(size_t) j * draw_stride + q];
-        } else if (any_logits && logits_out) {
+                for (int q = 0; q < ps.draw_stride; ++q) samp_out[(size_t) (r0 + j) * stride + q] = ps.hsamp[(size_t) j * ps.draw_stride + q];
+        } else if (ps.any_logits && logits_out) {
             for (int j = 0; j < n; ++j) if (rows[r0 + j].want_logits && logits_out[r0 + j])
                 memcpy(logits_out[r0 + j], hlogits + (size_t) j * V, (size_t) V * 4);
         }

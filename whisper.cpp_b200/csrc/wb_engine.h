@@ -102,11 +102,26 @@ struct Engine {
     DevBuf<int>    dints, xcnt;      // packed per-step integers: tokens | pos | cells | slot | n_kv | rowinfo[2] | capture index | idx[...]
     DevBuf<uint32_t> samp_mask;      // static suppression bit mask of the on-device sampler
     uint64_t samp_mask_key = 0;
-    DevBuf<SampOut> dsamp;           // [max_rows][SAMP_MAX_DRAWS]
-    SampOut * hsamp = nullptr;       // pinned, same shape
+    // A decode pass runs in one of PASS_SLOTS slots: its pinned row table, its sampler output (device and pinned) and the events around it.
+    // The pool keeps up to three passes in flight (a run-ahead pass, an ordinary pass behind it, the next run-ahead pass: wb_api.cpp,
+    // Group::run), so the host may fill one slot's table while the passes of the others are queued or running.  Device workspaces stay
+    // single: stream order serialises the passes.
+    static constexpr int PASS_SLOTS = 3;
+    struct PassSlot {
+        int * hints = nullptr;       // pinned mirror of dints for this pass
+        SampOut * hsamp = nullptr;   // pinned [max_rows][SAMP_MAX_DRAWS]
+        cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // around the pass; ev1 follows its device-to-host copy
+        bool busy = false;           // enqueued and not yet waited for
+        int n = 0, draw_stride = 1; bool any_logits = false;
+    };
+    PassSlot pslot[PASS_SLOTS];
+    DevBuf<SampOut> dsamp;           // [PASS_SLOTS][max_rows][SAMP_MAX_DRAWS]
+    SampOut * dsamp_of(int slot) const { return dsamp.p + (size_t) slot * max_rows * SAMP_MAX_DRAWS; }
+    SampOut * hsamp = nullptr;       // = pslot[slot].hsamp of the pass being enqueued
     DevBuf<double> ddraws; double * hdraws = nullptr;   // uniforms of the categorical draws of a pass [max_rows][stride] (device / pinned)
     int draw_stride = 1;             // entries per row of dsamp / ddraws in the current pass
-    int * hints = nullptr;           // pinned mirror of dints
+    int * hints = nullptr;           // = pslot[slot].hints of the pass being enqueued
+    int cur_slot = 0;
     float * hlogits = nullptr;       // pinned [8][n_vocab]
     int ld_idx = 0;
     // CUDA graphs of one decode pass, keyed by (rows, logits?, n_keys); rebuilt when buffers move
@@ -116,7 +131,7 @@ struct Engine {
     void drop_graphs();
 
     // device-event timers of the last encode: [1]=conv (incl. window staging) [2]=encoder [3]=cross  ([0] unused: mel is FrontEnd)
-    cudaEvent_t ev[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };   // [5],[6]: decode pass / k_dtw_qk; [6],[7]: DTW paths
+    cudaEvent_t ev[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };   // [5],[6]: k_dtw_qk; [6],[7]: DTW paths
     float last_ms[4] = { 0, 0, 0, 0 };
 
     ~Engine();
@@ -136,12 +151,19 @@ struct Engine {
     // (kv_idx[j*ld .. +n_kv[j]]) the cells it attends to.  logits_out[j]: host buffer of n_vocab floats for rows with want_logits.
     // The slots of the rows of one pass must hold cross K/V of the same context length (slot_n_ctx); a pass that mixes them is an error.
     // the kernels of one pass (<= max_rows rows) on `st`; every row's slot holds cross K/V of n_audio_ctx positions, n_keys = pad256 of it
-    bool decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp);
+    bool decode_pass_enqueue(int n, bool any_logits, int n_keys, int n_audio_ctx, const SampCfg * samp, bool tok_indirect = false);
     // samp != nullptr: logits stay on the device; the filter + greedy pick run there (rowinfo: 2 ints per row, samp_out: host [n_rows])
     bool decode(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, float * const * logits_out,
                 const SampCfg * samp = nullptr, const int * rowinfo = nullptr, SampOut * samp_out = nullptr,
                 const double * draws = nullptr, int stride = 1,    // draws: [n_rows][stride] uniforms (rows asking for categorical draws, rowinfo bits 8-14); samp_out: [n_rows][stride]
                 const int * cap_idx = nullptr);                    // per row: DTW capture index or -1 (null: no row is captured)
+    // The two halves of one pass of `decode` (n_rows <= max_rows): enqueue it into a free slot (returned in *slot) without waiting, and wait
+    // for it.  tok_src (may be null): per row -1, or the entry of dsamp (dsamp_of(s) + row of an earlier pass of slot s) whose token the row
+    // takes; that pass precedes this one in stream order, so its output is complete and is read before this pass's sampler runs.
+    // After pass_wait(slot) the pass's sampler output is pslot[slot].hsamp until the slot is enqueued again.
+    bool pass_enqueue(const DecToken * rows, int n_rows, const int * cells, const int * kv_idx, int ld, const int * n_kv, const SampCfg * samp,
+                      const int * rowinfo, const double * draws, int stride, const int * cap_idx, const int * tok_src, int * slot);
+    bool pass_wait(int slot);
     bool set_samp_mask(uint64_t key, const std::vector<uint32_t> & bits);
 };
 

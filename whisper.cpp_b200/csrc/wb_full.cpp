@@ -425,6 +425,16 @@ void samp_rowinfo(const Vocab & vocab, const whisper_full_params & params, const
     out2[0] = f; out2[1] = d.seek_delta / 2;
 }
 
+// samp_rowinfo of the step after the one being submitted, were the token sampled now a text token (< token_beg) appended to `d`
+void samp_rowinfo_next(const Vocab & vocab, const whisper_full_params & params, const Decoder & d, int * out2) {
+    const auto & cur = d.sequence.tokens;
+    int f = 0;
+    if (cur.empty() || cur.back().id >= vocab.token_beg) f |= 4;
+    if (d.has_ts) f |= 8;
+    if (!params.no_timestamps && !params.single_segment && params.max_tokens > 0 && (int) cur.size() + 1 >= params.max_tokens) f |= 16;
+    out2[0] = f; out2[1] = d.seek_delta / 2;
+}
+
 // P(no-speech token) exactly as whisper.cpp:7190-7200 computes it: row 0 of the logits buffer, normalised with the log-sum-exp that
 // whisper_compute_logprobs (whisper.cpp:6156-6176) forms against the maximum of the WHOLE buffer (see whisper_state::lrows)
 float row0_nosp(const whisper_context & ctx, const whisper_state & st) {
@@ -646,6 +656,14 @@ WB_EXPORT int whisper_full_with_state(struct whisper_context * ctx, struct whisp
         make_samp_cfg(*ctx, params, sreq.cfg);
     }
 
+    // run-ahead (SampReq::next_step): whether step i of the loop below submits a decode for `d` when the token it samples is a text token
+    // (neither end-of-text nor a timestamp): not if max_tokens, the loop or the end of the audio ends the sequence there, or its last
+    // step fails it
+    const int n_max_steps = n_text_ctx / 2 - 4;
+    auto step_follows = [&](const Decoder & d, int i) {
+        if (i >= n_max_steps || (params.max_tokens > 0 && i >= params.max_tokens) || (d.has_ts && seek + d.seek_delta + delta_min >= seek_end)) return false;
+        return i < n_max_steps - 1 || (d.sequence.result_len != 0 && d.seek_delta >= 100 * WB_CHUNK_SIZE / 2);
+    };
     struct BeamCand { int decoder_idx; int seek_delta; bool has_ts; Sequence sequence; Grammar grammar; };
     std::vector<std::vector<BeamCand>> bc_per_dec(n_decoders);
     std::vector<BeamCand> cands;
@@ -719,6 +737,8 @@ WB_EXPORT int whisper_full_with_state(struct whisper_context * ctx, struct whisp
                 for (int j = 0; j < n_cur; ++j) { Decoder & d = state->decoders[j]; d.have_pending = false; d.have_pending_k = false; d.predrawn.clear(); }
                 sreq.draws = nullptr; sreq.stride = 1;
                 if (dev_samp) { rowinfo.assign((size_t) 2 * np, 0); samp_rowinfo(vocab, params, state->decoders[0], &rowinfo[2 * (np - 1)]); sreq.rowinfo = rowinfo.data(); }
+                sreq.next_step = dev_samp && !dev_beam && n_cur == 1 && step_follows(state->decoders[0], 0);      // step 0 of the loop below
+                if (sreq.next_step) samp_rowinfo_next(vocab, params, state->decoders[0], sreq.next_rowinfo);
                 if (dev_beam) {      // every decoder draws its k candidates from the distribution of the prompt's last row, each with its own generator (whisper.cpp:7212-7221, 7270-7290)
                     const int nd = n_cur * bk;
                     draws.assign((size_t) np * nd, 0.0);
@@ -874,6 +894,8 @@ WB_EXPORT int whisper_full_with_state(struct whisper_context * ctx, struct whisp
                         for (int j = 0; j < n_cur; ++j) { const Decoder & d = state->decoders[j]; if (!(d.failed || d.completed)) samp_rowinfo(vocab, params, d, &rowinfo[2 * d.i_batch]); }
                         sreq.rowinfo = rowinfo.data();
                     }
+                    sreq.next_step = dev_samp && !dev_beam && n_cur == 1 && step_follows(state->decoders[0], i + 1);
+                    if (sreq.next_step) samp_rowinfo_next(vocab, params, state->decoders[0], sreq.next_rowinfo);
                     if (dev_beam) {
                         draws.assign(b_tok.size() * (size_t) bk, 0.0);
                         for (int j = 0; j < n_cur; ++j) {

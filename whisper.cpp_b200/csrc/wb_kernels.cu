@@ -558,6 +558,13 @@ __global__ void k_dec_embed(const QMat te, const float * __restrict__ pe, const 
 void dec_embed(const QMat & te, const float * pe, const int * tokens, const int * pos, int n_tok, int d, float * x, cudaStream_t st) {
     k_dec_embed<<<n_tok, 256, 0, st>>>(te, pe, tokens, pos, d, x); count_launch();
 }
+__global__ void k_tok_resolve(int * __restrict__ tok, const SampOut * __restrict__ samp, int n_tok) {
+    const int t = threadIdx.x;
+    if (t < n_tok && tok[t] < 0) tok[t] = samp[-1 - tok[t]].id;
+}
+void tok_resolve(int * tokens, const SampOut * samp, int n_tok, cudaStream_t st) {
+    k_tok_resolve<<<1, 64 * ((n_tok + 63) / 64), 0, st>>>(tokens, samp, n_tok); count_launch();
+}
 __global__ void k_dequant_rows(const QMat W, float * __restrict__ out) {
     const int64_t n = (int64_t) W.N * W.K;
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x)

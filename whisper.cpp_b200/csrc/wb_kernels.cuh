@@ -97,5 +97,7 @@ struct SampOut { int id, tid; float p, plog, pt, ptsum, nosp_raw;
 void greedy_sample(const float * logits, int V, int n, const int * rowinfo, const SampCfg & cfg, SampOut * out, cudaStream_t st,
                    const double * draws = nullptr, int stride = 1);
 constexpr int SAMP_MAX_DRAWS = 64;
+// tokens[t] < 0 is replaced by samp[-1 - tokens[t]].id: a row whose token is the pick of an earlier pass's sampler (run-ahead passes)
+void tok_resolve(int * tokens, const SampOut * samp, int n_tok, cudaStream_t st);
 
 } // namespace wb

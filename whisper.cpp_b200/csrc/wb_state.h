@@ -138,6 +138,7 @@ struct whisper_context {
     bool scripted = false;                     // TEST HOOK: see whisper_state::scripted
     std::vector<std::pair<int, int>> dtw_heads; // (text layer, head) of the alignment heads when params.dtw_token_timestamps survived init
     std::unique_ptr<wb::Group> pool;           // device pool shared by every state of this context (created with the first state)
+    bool run_ahead = true;                     // TEST HOOK (wb200_dbg_run_ahead): Group::run_ahead of the pools created for this context
     // In-library multi-GPU: with WB200_DEVICES=all (or a list "0,1,..") a context loaded from a FILE keeps one replica of the weights per
     // listed GPU.  whisper_init_state places each new state on the GPU that holds the fewest, so whisper_full_parallel and concurrent
     // whisper_full_with_state callers spread over the box without any change on their side; every GPU batches its own states (no
@@ -158,7 +159,10 @@ namespace wb {
 // once per step).  A state that runs alone gets a 1-row pass immediately.
 // request for the on-device logits filter + greedy pick of the rows of one decode call
 struct SampReq { SampCfg cfg; uint64_t mask_key = 0; const std::vector<uint32_t> * mask_bits = nullptr; const int * rowinfo = nullptr;
-                 const double * draws = nullptr; int stride = 1; };   // beam search: [n_rows][stride] uniforms for the categorical draws; samp_out then holds `stride` entries per row
+                 const double * draws = nullptr; int stride = 1;      // beam search: [n_rows][stride] uniforms for the categorical draws; samp_out then holds `stride` entries per row
+                 // run-ahead (Group::run): the member will submit the single-token step that follows the request's last row if the token
+                 // sampled there is a text token, and that step's rowinfo will be next_rowinfo
+                 bool next_step = false; int next_rowinfo[2] = { 0, 0 }; };
 
 struct Group {
     Engine eng;
@@ -194,6 +198,22 @@ struct Group {
         bool ok = false; int64_t dt_us = 0;
     };
     std::vector<Req *> pending;
+    // ---- run-ahead: after a pass of greedy, device-sampled rows the pool enqueues the next single-token step of every sequence that may
+    // continue, with the token taken from the pass's sampler output on the device and every other input predicted on the host.  The next
+    // batch takes the results of the rows whose real request equals the prediction; the others run in an ordinary pass.  A rejected row
+    // is harmless: it wrote K/V only into the cell predicted for its own state, which no pass attends to before the pass that allocates
+    // it writes it again, and that pass comes later in stream order.
+    struct SpecRow {
+        const whisper_state * st; int token, pos, seq, slot, cell, n_ctx, rowinfo[2];   // token: filled in when its source pass is waited for
+        std::vector<int> idx;                    // attended cells
+        int src_pass, src_row;                   // pass slot and row of the sampler output that holds the token
+    };
+    int spec_pass = -1;                         // engine pass slot of the queued run-ahead pass, -1: none
+    uint64_t spec_mask_key = 0; SampCfg spec_cfg;
+    std::vector<SpecRow> spec_rows;
+    float spec_miss = 0.0f; int spec_idle = 0;  // share of recent run-ahead batches with a mispredicted row; batches since the last run-ahead pass
+    bool run_ahead = true;                      // test hook (wb200_dbg_run_ahead): false keeps every batch on the lock-step path
+    void spec_drop();                           // wait for the queued run-ahead pass and forget it (no batch is running)
     void enter(whisper_state * st);             // the state starts issuing requests (whisper_full_with_state, or one low-level call)
     void leave(whisper_state * st);
     void suspend(whisper_state * st);           // the state's thread is busy with a nested call on another state
